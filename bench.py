@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- decode tokens/s of a synthetic Llama-3-8B "v8-k65536-256" VPTQ stack on N B200s.
+"""bench.py -- decode tokens/s of a synthetic Llama-3-8B "v8-k65536-256" VPTQ stack on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
 
 One step = one decode token (batch 1) through every VPTQ-quantized linear of Llama-3-8B:
 32 layers x (q 4096x4096, k/v 1024x4096, o 4096x4096, gate/up 14336x4096, down 4096x14336),
@@ -10,7 +10,7 @@ perm + norm enabled -- 224 fused GEMV launches chained by true data dependence
 (h -> q,k,v ; q -> o ; o -> gate,up ; gate -> down -> next layer).  Attention, norms, the
 fp16 embedding and lm_head are NOT on the VPTQ path and are not executed (stated in `config`).
 Weights are synthetic (uniform random packed indices, random codebooks); 2.6 GB of indices per
-token stream from HBM every step, ~20x the L2.
+token stream from HBM every step, ~50x the L2.
 
 Printed JSON (one line, rank 0): the driver contract + `roofline`, `cpu_baseline`, `e2e`, `clocks`.
   value     tokens/s, inputs resident in HBM, one CUDA graph of the 224 launches per step
@@ -18,6 +18,8 @@ Printed JSON (one line, rank 0): the driver contract + `roofline`, `cpu_baseline
   roofline  HBM: algorithmic bytes (packed indices + x + y of every launch) / step time
   N > 1     tensor-parallel over out_features; exchange fused into the GEMV over NVLink peer memory (tagged words;
             --tp-mode nccl: one NCCL all-reduce per launch, the north_star form), strong scaling; `tp_check`
+--dump-outputs DIR writes the final hidden state of the last timed step as DIR/hidden.npy (float32): inputs and
+weights are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -71,7 +73,7 @@ def algorithmic_bytes(m, q, tokens=1, world=1):
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md recipe)
+# clocks sampling: nvidia-smi queried every 100 ms during the timed region
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -539,6 +541,10 @@ def run_ours(args):
             tp_err = int(te.item())
         assert tp_err == 0, "a tensor-parallel flag wait timed out"
         h_final = h_out.clone()
+        if args.dump_outputs and rank == 0:
+            import numpy as np
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "hidden.npy"), h_final.float().cpu().numpy())
 
         # ---- `e2e`: host buffers, H2D + D2H inside the timed region, per-step sync ------------------
         e2e_steps = args.steps
@@ -592,16 +598,10 @@ def run_ours(args):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        peak = float(peaks.get("hbm_gbs", 6650.0))
+        peak = float(peaks.get("hbm_gbs", 3350.0))
         abytes = algorithmic_bytes(m, q, 1, world)         # per rank and step
         achieved = abytes / (ms_step * 1e-3) / 1e9
-        traffic = None
         uses_lists = lists_on
-        try:
-            tj = json.load(open(os.path.join(ROOT, "profiles", "gemv_traffic.json")))
-            traffic = (tj["lists"] if uses_lists else tj)["dram_bytes_per_token"] // (n_launch * world)
-        except Exception:
-            pass
         line = {
             "metric": metric, "value": round(value, 2), "unit": "tokens/s", "n_gpus": world, "steps": args.steps,
             "warmup": max(args.warmup, 3), "ms_per_step": round(ms_step, 4), "higher_is_better": True,
@@ -626,15 +626,14 @@ def run_ours(args):
                     "h2d_bytes_per_step": x_host.numel() * 2, "d2h_bytes_per_step": y_host.numel() * 2,
                     "wall_ms_per_step": round(wall_e2e / e2e_steps, 4)},
             "roofline": {"bound": "hbm", "achieved": round(achieved, 1), "peak": peak, "unit": "GB/s",
-                         "frac": round(achieved / peak, 4), "traffic": traffic,
-                         "traffic_source": "ncu dram__bytes_read+write per launch, profiles/gemv_traffic.json (one --set full "
-                                           "capture per shape, profiles/r02_ncu_shapes_metrics.csv); not measured in this run",
+                         "frac": round(achieved / peak, 4),
                          "kernel": ("gemv_lists_kernel<half,true> (csrc/gemv_lists.cu: 64 KiB codebook slices in shared "
                                     "memory, slice x tile index lists)") if uses_lists else
                                    "gemv_body<half,8,1,false,true> (entry points gemv_kernel / gemv_multi_kernel)",
                          "algorithmic_bytes_per_launch": abytes // n_launch,
                          "avg_launch_us": round(ms_step * 1e3 / n_launch, 3),
-                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else "fallback 6650 (of fallback)"},
+                         "peak_source": "MEASURED_PEAKS.json hbm_gbs (of measured)" if peaks else
+                                        "H100 SXM data sheet, 3350 GB/s HBM3 (not reached)"},
             "clocks": clk,
         }
         # resident bytes of this rank's weights: checkpoint tensors + load-time index lists of the decode kernel
@@ -757,13 +756,13 @@ def run_reference(args):
 
 # ------------------------------------------------------------------------------------------------
 # GPU-vs-GPU bar: the reference's OWN CUDA kernels (oracle/_ref/libvptq.so, unmodified sources compiled for
-# sm_100a by oracle/build_ref.sh) timed on the same box, eager, one launch pair per linear as the reference runs
+# sm_90a by oracle/build_ref.sh) timed on the same GPU, eager, one launch pair per linear as the reference runs
 # them (csrc/quant_gemv.cu:241-294 + its sum(-1) epilogue; prefill: csrc/dequant.cu:227-287 + F.linear).
 # ------------------------------------------------------------------------------------------------
 def prefill_timing(m, q, stack, device, dtype, tokens=8192):
     """BASELINE.json configs[2] (prefill, batch 4 x seq 2048 = 8192 tokens) on the three distinct linear shapes of one
-    decoder layer: vptq_b200_quant_gemm (prep + dequant into the workspace + hand-written tcgen05 GEMM) next to OUR
-    dequant kernel + cuBLAS through torch, and the tensor-pipe share of the bf16 sustained peak."""
+    decoder layer: vptq_b200_quant_gemm (prep + dequant into the workspace + hand-written wgmma GEMM) next to OUR
+    dequant kernel + cuBLAS through torch, and the share of the dense 16-bit tensor-core peak."""
     import torch
     from vptq_b200 import native
     peaks = {}
@@ -771,7 +770,7 @@ def prefill_timing(m, q, stack, device, dtype, tokens=8192):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("bf16_tflops_sustained", 1436.0))
+    peak = float(peaks.get("bf16_tflops_sustained", 989.0))
     out = {"tokens": tokens, "shapes": {}}
     for name in ("q", "gate", "down"):
         t = stack[0][name]
@@ -795,11 +794,12 @@ def prefill_timing(m, q, stack, device, dtype, tokens=8192):
             torch.nn.functional.linear(x, W)
         cub = med(deq_cublas)
         tf = 2.0 * tokens * i * o / (ours * 1e-3) / 1e12
-        out["shapes"][f"{name}_{o}x{i}"] = {"ms": round(ours, 4), "tflops": round(tf, 1), "frac_of_bf16_sustained": round(tf / peak, 3),
+        out["shapes"][f"{name}_{o}x{i}"] = {"ms": round(ours, 4), "tflops": round(tf, 1), "frac_of_peak": round(tf / peak, 3),
                                             "our_dequant_plus_cublas_ms": round(cub, 4)}
         del x, y, W
     out["how"] = ("median of 7, CUDA events, whole op (x' prep + dequant + GEMM); flops = 2*T*I*O; peak = "
-                  "MEASURED_PEAKS.json bf16_tflops_sustained")
+                  + ("MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else
+                     "H100 SXM data sheet, 989 TFLOP/s dense 16-bit (not reached)"))
     return out
 
 
@@ -887,6 +887,8 @@ def main():
     ap.add_argument("--debug-layers", type=int, default=0, help="debugging only: truncate the model (invalid as a result)")
     ap.add_argument("--model", default="llama3-8b", choices=sorted(MODELS))
     ap.add_argument("--no-check", action="store_true", help="skip the unsharded recomputation of the token")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the final hidden state of the last timed step to DIR/hidden.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 /*
- * vptq_b200.h  --  C ABI of libvptq_b200.so: the B200 (sm_100a) VPTQ quantized-linear hot path.
+ * vptq_b200.h  --  C ABI of libvptq_b200.so: the H100 (sm_90a) VPTQ quantized-linear hot path.
  *
  * This is the drop-in boundary.  It replaces the three pybind11 entry points the reference
  * registers in csrc/ops.cc:44-55 (module `vptq.libvptq`, bound by vptq/ops/quant_gemm.py:22-26):
@@ -11,7 +11,7 @@
  *   dequant      = vptq::dequant                           vptq_b200_dequant
  *                  csrc/ops.cc:9-18,47   dequant.cu:227
  *   dequant + torch F.linear (vptq/ops/quant_gemm.py:231-275)
- *                                                          vptq_b200_quant_gemm   (fused, tcgen05)
+ *                                                          vptq_b200_quant_gemm   (fused, wgmma)
  *   quant_gemv_v2 = vptq::quant_gemv_v2                    vptq_b200_quant_gemv_v2
  *                  csrc/ops.cc:32-38,53  quant_gemv_v2.cu:25
  *
@@ -62,7 +62,7 @@ typedef enum vptq_status {
   VPTQ_ERR_UNSUPPORTED = -2, /* well-formed but not implemented (message says what)        */
   VPTQ_ERR_WORKSPACE = -3,   /* workspace smaller than vptq_b200_workspace_bytes()         */
   VPTQ_ERR_CUDA = -4,        /* a CUDA runtime call failed (message carries the CUDA text) */
-  VPTQ_ERR_DEVICE = -5       /* current device is not compute capability 10.x              */
+  VPTQ_ERR_DEVICE = -5       /* current device is not compute capability 9.0               */
 } vptq_status;
 
 /* launch flags (bit-or) */
@@ -291,8 +291,8 @@ VPTQ_B200_API int vptq_b200_dequant(const vptq_linear_desc* desc, void* w_out, v
 /*
  * Prefill path: y = x W^T + bias for many tokens (replaces dequant + torch F.linear,
  * vptq/ops/quant_gemm.py:231-275): the quantised weight is dequantised once into the workspace (16-bit,
- * quantised column order, scale / bias / perm kept out of it) and fed by TMA to a tcgen05 tensor-core
- * GEMM with TMEM accumulators.
+ * quantised column order, scale / bias / perm kept out of it) and fed by TMA to a wgmma tensor-core
+ * GEMM with register accumulators.
  */
 VPTQ_B200_API int vptq_b200_quant_gemm(const vptq_linear_desc* desc, const void* x, int64_t x_stride, void* y,
                          int64_t y_stride, int32_t tokens, void* workspace,

@@ -3,9 +3,9 @@
 #
 # Compiles the UNMODIFIED reference CUDA extension (csrc/quant_gemv.cu, csrc/dequant.cu,
 # csrc/quant_gemv_v2.cu, csrc/ops.cc) from where it lies under /root/reference into
-# oracle/_ref/libvptq.so for sm_100a, bypassing the reference's CMake (which needs the legacy
+# oracle/_ref/libvptq.so for sm_90a, bypassing the reference's CMake (which needs the legacy
 # FindCUDA macros and pins the pre-C++11 ABI; see DESIGN.md "oracle/_ref").
-# Outputs go ONLY to oracle/_ref/ (git-ignored; travels to the GPU box with gpurun).
+# Outputs go ONLY to oracle/_ref/ (git-ignored build products).
 # No reference source is copied into this repository.
 set -euo pipefail
 REF=${REF:-/root/reference}
@@ -21,7 +21,7 @@ NVFLAGS=(-I"$REF/csrc" -I"$REF/third_party/cutlass/include" -I"$T/include"
   -U__CUDA_NO_HALF_OPERATORS__ -U__CUDA_NO_HALF_CONVERSIONS__ -U__CUDA_NO_HALF2_OPERATORS__
   -U__CUDA_NO_BFLOAT16_OPERATORS__ -U__CUDA_NO_BFLOAT16_CONVERSIONS__
   -U__CUDA_NO_BFLOAT162_OPERATORS__ -U__CUDA_NO_BFLOAT162_CONVERSIONS__
-  -gencode arch=compute_100a,code=sm_100a)
+  -gencode arch=compute_90a,code=sm_90a)
 pids=()
 for tu in quant_gemv quant_gemv_v2 dequant; do
   if [ ! -f "$OUT/obj/$tu.o" ]; then

@@ -1,4 +1,4 @@
-"""bench.py: the arithmetic behind the reported roofline (CPU only; the timed legs need a B200)."""
+"""bench.py: the arithmetic behind the reported roofline (CPU only; the timed legs need an H100)."""
 import json
 import os
 import sys
@@ -34,10 +34,3 @@ def test_models_are_the_baseline_configs():
     s = bench.workload_string(m8, q8, cfg8)
     assert "224 VPTQ linears" in s and "(b=24)" in s
 
-
-def test_traffic_file_has_both_kernels():
-    tj = json.load(open(os.path.join(ROOT, "profiles", "gemv_traffic.json")))
-    assert tj["dram_bytes_per_token"] > 0 and tj["lists"]["dram_bytes_per_token"] > 0
-    m, q, _, _ = bench.MODELS["llama3-8b"]
-    ratio = tj["lists"]["dram_bytes_per_token"] / bench.algorithmic_bytes(m, q)
-    assert 1.0 < ratio < 1.6          # 4-byte entries + padding + codebooks: 1.52x measured

@@ -1,4 +1,4 @@
-"""GPU parity of the prefill path (tokens >= 3): prep kernel + quantised-order dequant + tcgen05 GEMM,
+"""GPU parity of the prefill path (tokens >= 3): prep kernel + quantised-order dequant + wgmma GEMM,
 through VQuantLinear.forward -> vptq.ops.quant_gemm -> C ABI, against the oracle.
 
 Bar: max|y - y*| / max|y*| <= 1e-3 (fp16), 4e-3 (bf16); y* = fp64-accumulated math on the identical

@@ -1,4 +1,4 @@
-"""Prefill timing: our fused path (prep + dequant + tcgen05 GEMM) vs torch (cuBLAS) on the same dequantised weight."""
+"""Prefill timing: our fused path (prep + dequant + wgmma GEMM) vs torch (cuBLAS) on the same dequantised weight."""
 import os, sys, json
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in (ROOT, os.path.join(ROOT, "oracle"), os.path.join(ROOT, "tests")):

@@ -1,6 +1,6 @@
 // Gather-tier microbenchmark for the VPTQ GEMV design (SURVEY.md 7.4 H1): how many random
-// 16-byte codebook gathers per second does each tier of a B200 deliver, next to plain HBM streaming?
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gather_microbench tools/gather_microbench.cu
+// 16-byte codebook gathers per second does each tier of an H100 deliver, next to plain HBM streaming?
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o gather_microbench tools/gather_microbench.cu
 // Prints one JSON object per experiment.
 #include <cuda_runtime.h>
 #include <cooperative_groups.h>

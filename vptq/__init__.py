@@ -2,7 +2,7 @@
 
 Hugging Face transformers imports the quantized layer as `from vptq import VQuantLinear`
 (transformers/integrations/vptq.py); putting this repository on sys.path makes that import land
-on the B200 implementation without touching transformers.
+on the H100 implementation without touching transformers.
 """
 import sys
 

@@ -1,4 +1,4 @@
-"""vptq_b200: the VPTQ quantized-linear hot path, written from scratch for NVIDIA B200 (sm_100a).
+"""vptq_b200: the VPTQ quantized-linear hot path, written from scratch for NVIDIA H100 (sm_90a).
 
 Public surface = the reference's (vptq/__init__.py:7-15): `VQuantLinear`, `ops`, `__version__`.
 """

@@ -1,9 +1,9 @@
-"""Build libvptq_b200.so in-tree with nvcc for sm_100a (no CMake, no pybind, no torch headers).
+"""Build libvptq_b200.so in-tree with nvcc for sm_90a (H100; no CMake, no pybind, no torch headers).
 
     python -m vptq_b200.build [--force] [--verbose]
 
-The shared library is written next to this file (vptq_b200/libvptq_b200.so): it is git-ignored
-but travels to the GPU box with the repository snapshot.  nvcc cross-compiles without a GPU.
+The shared library is written next to this file (vptq_b200/libvptq_b200.so, git-ignored).  nvcc
+cross-compiles without a GPU.
 """
 from __future__ import annotations
 
@@ -20,9 +20,10 @@ INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libvptq_b200.so")
 
-SOURCES = ["api.cu", "gemv.cu", "gemv_inst_v8.cu", "gemv_inst_vx.cu", "gemv_lists.cu", "lists_build.cu", "dequant.cu", "gemv_v2.cu", "gemm_tcgen05.cu"]
+SOURCES = ["api.cu", "gemv.cu", "gemv_inst_v8.cu", "gemv_inst_vx.cu", "gemv_lists.cu", "lists_build.cu", "dequant.cu", "gemv_v2.cu", "gemm_wgmma.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = (["-DVPTQ_B200_PROF_WARPS"] if os.environ.get("VPTQ_B200_PROF_WARPS") else []) + ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = (["-DVPTQ_B200_PROF_WARPS"] if os.environ.get("VPTQ_B200_PROF_WARPS") else []) + [*ARCH, "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -74,7 +75,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
         with cf.ThreadPoolExecutor(max_workers=min(len(jobs), os.cpu_count() or 4)) as ex:
             list(ex.map(compile_one, jobs))
     if jobs or not os.path.exists(LIB):
-        cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a",
+        cmd = [NVCC, "-shared", "-o", LIB, *objs, *ARCH,
                "-Xcompiler", "-fPIC", "-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:

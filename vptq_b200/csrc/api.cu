@@ -137,8 +137,8 @@ int validate(const vptq_linear_desc* d, bool need_device) {
   if (need_device) {
     const DeviceInfo* dev = device_info();
     if (!dev) return VPTQ_ERR_CUDA;
-    if (dev->cc_major != 10) {
-      set_error("device compute capability %d.%d: this library contains sm_100a code only", dev->cc_major,
+    if (dev->cc_major != 9 || dev->cc_minor != 0) {
+      set_error("device compute capability %d.%d: this library contains sm_90a code only", dev->cc_major,
                 dev->cc_minor);
       return VPTQ_ERR_DEVICE;
     }
@@ -171,12 +171,12 @@ size_t vptq_b200_workspace_bytes(const vptq_linear_desc* desc, int32_t tokens, i
   switch (op) {
     case VPTQ_OP_GEMV: {
       if (!desc->indices) return gemv_lists_workspace_bytes(*desc);
-      // exact for the current device; without one (CPU-only host) the B200 geometry is assumed
-      DeviceInfo b200;
-      b200.sm_count = 148, b200.smem_optin = 232448, b200.cc_major = 10;
+      // exact for the current device; without one (CPU-only host) the H100 SXM geometry is assumed
+      DeviceInfo h100;
+      h100.sm_count = 132, h100.smem_optin = 232448, h100.cc_major = 9;
       const DeviceInfo* dev = device_info();
       GemvPlan pl;
-      if (gemv_make_plan(*desc, tokens, dev ? *dev : b200, &pl)) return 0;
+      if (gemv_make_plan(*desc, tokens, dev ? *dev : h100, &pl)) return 0;
       return std::max(pl.ws_counters_bytes + pl.ws_partials_bytes, gemv_lists_workspace_bytes(*desc));
     }
     case VPTQ_OP_DEQUANT: return dequant_workspace_bytes(*desc);
@@ -322,8 +322,8 @@ int vptq_b200_quant_gemv_v2(int32_t dtype, const void* x, void* y, int32_t token
   }
   const DeviceInfo* dev = device_info();
   if (!dev) return VPTQ_ERR_CUDA;
-  if (dev->cc_major != 10) {
-    set_error("device compute capability %d.%d: sm_100a code only", dev->cc_major, dev->cc_minor);
+  if (dev->cc_major != 9 || dev->cc_minor != 0) {
+    set_error("device compute capability %d.%d: sm_90a code only", dev->cc_major, dev->cc_minor);
     return VPTQ_ERR_DEVICE;
   }
   GemvV2Args a{dtype,     tokens,           in_features,     out_features,       vector_len,    num_centroids,

@@ -145,7 +145,7 @@ int gemv_make_plan(const vptq_linear_desc& d, int tokens, const DeviceInfo& dev,
     // ---- column chunks (cpg per codebook group, multiples of 128 columns) x warps per row -------
     // A CTA streams rows_cta * cc fields; its nwarps/wsplit row slots work in parallel, each row
     // cut over wsplit warps.  Chunk counts up to 8 reduce through a cluster (the co-schedulable
-    // cluster count can leave SMs idle: 4-CTA clusters fill only 132 of 148 SMs), more than 8
+    // cluster count can leave SMs idle: a cluster must fit inside one GPC), more than 8
     // through global memory.
     GemvKernelFn fn_probe = pick_kernel(d, pl.nt, a.main_smem);
     int best_cpg = 0, best_cc = 0, best_ws = 1;

@@ -3,9 +3,9 @@
 // time by vptq_b200/lists.py or vptq_b200_lists_build_host).
 //
 // The generic kernel (gemv_kernel.cuh) gathers such a codebook through L1/L2 and is bound by the L1TEX tag
-// stage at ~1.1 gathers/clk/SM (profiles/r01_gather_microbench.jsonl), 14 % of the HBM roofline at best.
-// Here every gather is a shared-memory access, and -- unlike the round-1 sliced kernel this file replaces --
-// there is no cluster (all 148 SMs work), no perm / dependent gather in the prologue, a 4-byte entry, and the
+// stage, far below the HBM roofline.
+// Here every gather is a shared-memory access, and there is no cluster (every SM works), no perm / dependent
+// gather in the prologue, a 4-byte entry, and the
 // x' tile is bounded by 4096 columns, so any in_features fits:
 //   * work item = unit u = (tile t, slice s, index row r): the fields of row r whose main index lies in slice
 //     s (64 KiB of the codebook) and whose ORIGINAL input feature lies in column tile t (<= 4096 features).
@@ -20,7 +20,7 @@
 //     compile-time position: five straight-line batch variants, no per-step test); per
 //     entry a lane does LDS.32 (entry), LDS.128 (main), LDS.128 (residual), LDS.U16 (x'), then c + r in
 //     packed 16-bit arithmetic (exactly the reference's ADD2, csrc/kernels/quant_gemv.cuh:124-127) and 8
-//     mixed-precision FMAs into fp32 accumulators (fma.rn.f32.f16 -> SASS FHFMA);
+//     FMAs into fp32 accumulators;
 //   * a unit that lies inside one warp's run is reduced with 9 shuffles; the (at most two) units a run shares
 //     with its neighbours are parked in shared memory and merged in warp order;
 //   * reduction over the Q = NS * NT combos of a row: every unit adds its 8 sums, converted to 2^-30 fixed
@@ -130,23 +130,18 @@ __device__ __forceinline__ void red_add_fixed(unsigned long long* p, float v) {
   const long long q = __float2ll_rn(v * kFixScale);
   asm volatile("red.global.add.u64 [%0], %1;" ::"l"(p), "l"(q) : "memory");
 }
-// sm_100 mixed-precision FMA (SASS FHFMA): fp16 x fp16 + fp32 -> fp32, the product is exact
-__device__ __forceinline__ float fma_f32_f16(uint16_t a, uint16_t b, float c) {
-  float r;
-  asm("fma.rn.f32.f16 %0, %1, %2, %3;" : "=f"(r) : "h"(a), "h"(b), "f"(c));
-  return r;
-}
-
-// acc[e] += x' * (c[e] + r[e]).  fp16: c + r in packed fp16 (the reference's ADD2), fp32 accumulation.
+// acc[e] += x' * (c[e] + r[e]).  fp16: c + r in packed fp16 (the reference's ADD2), fp32 accumulation: the
+// fp16 x fp16 product is exact in fp32, so widening both factors and one fp32 FMA round exactly once.
 // bf16: c + r and the product in fp32 (x' is kept as fp16 in shared memory for both dtypes).
 template <typename T, bool RES>
 __device__ __forceinline__ void fma_entry(float (&acc)[8], uint16_t xh, const uint32_t (&cw)[4], const uint32_t (&rw)[4]) {
   if constexpr (std::is_same<T, __half>::value) {
+    const float xv = __half2float(__ushort_as_half(xh));
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
-      const uint32_t s = RES ? DT<T>::add2(cw[i], rw[i]) : cw[i];
-      acc[2 * i] = fma_f32_f16(xh, uint16_t(s & 0xffffu), acc[2 * i]);
-      acc[2 * i + 1] = fma_f32_f16(xh, uint16_t(s >> 16), acc[2 * i + 1]);
+      const float2 c = DT<T>::unpack2(RES ? DT<T>::add2(cw[i], rw[i]) : cw[i]);
+      acc[2 * i] = fmaf(xv, c.x, acc[2 * i]);
+      acc[2 * i + 1] = fmaf(xv, c.y, acc[2 * i + 1]);
     }
   } else {
     const float xv = __half2float(__ushort_as_half(xh));

@@ -114,7 +114,7 @@ int dequant_launch(const vptq_linear_desc& d, void* w_out, void* workspace, size
 bool dequant_orig_fast_ok(const vptq_linear_desc& d, const void* w_out, int64_t ld);  // 8-columns-per-thread path applies
 
 // -------------------------------------------------------------------------------------------
-// prefill GEMM (tcgen05)
+// prefill GEMM (wgmma)
 // -------------------------------------------------------------------------------------------
 size_t gemm_workspace_bytes(const vptq_linear_desc& d, int tokens);
 int gemm_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void* y, int64_t y_stride,

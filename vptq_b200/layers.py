@@ -1,4 +1,4 @@
-"""`VQuantLinear`: the VPTQ quantized linear module on the B200 CUDA path.
+"""`VQuantLinear`: the VPTQ quantized linear module on the H100 CUDA path.
 
 Drop-in for the reference module (vptq/layers/vqlinear.py:17-240): same constructor signature
 (:56-75), same parameter / sub-module names, shapes and storage dtypes -- i.e. the same
@@ -14,7 +14,7 @@ public VPTQ-community checkpoints load unchanged:
     perm                      [I]                            int16 view of uint16 (packed) | int64
     weight_scale, weight_bias [I],   bias [O]
 
-`forward` hands these tensors to `vptq_b200.ops.quant_gemm`, which runs the sm_100a kernels.
+`forward` hands these tensors to `vptq_b200.ops.quant_gemm`, which runs the sm_90a kernels.
 The constructor is meta-device safe (HF builds the module under `torch.device("meta")`).
 """
 from __future__ import annotations

@@ -4,7 +4,7 @@ Format contract: include/vptq_b200.h (`vptq_linear_desc::lists_stream`, `::lists
 `::lists_tile_cols`); consumer: vptq_b200/csrc/gemv_lists.cu.
 
 Why.  A main codebook of K = 65536 entries (1 MiB) cannot sit in one SM's shared memory, and gathering
-it through L1/L2 is bound by the L1TEX tag stage at ~1.1 gathers/clk/SM (profiles/r01_gather_microbench).
+it through L1/L2 is bound by the L1TEX tag stage.
 A sum does not care about the order of its terms, so the fields of every index row are re-bucketed:
 
   * the codebook is cut into NS = K / 4096 slices of 64 KiB (a 12-bit index inside a slice);

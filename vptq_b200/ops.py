@@ -1,13 +1,13 @@
-"""`vptq.ops` operator surface on the B200 CUDA path.
+"""`vptq.ops` operator surface on the H100 CUDA path.
 
 Function names, argument order and argument meaning are the reference's
 (vptq/ops/quant_gemm.py: `dequant` :43-69, `quant_gemm` :161-187, `quant_gemv_v2` :278-292), so
 `VQuantLinear.forward` and the reference's tests can call them unchanged.  What differs:
 
-* every op runs hand-written sm_100a CUDA through the C ABI (vptq_b200.native); there is no
+* every op runs hand-written sm_90a CUDA through the C ABI (vptq_b200.native); there is no
   torch implementation to fall back to -- CPU tensors raise;
 * routing: fewer than 3 tokens -> fused GEMV (the reference's rule, :213); otherwise the fused
-  dequant->tcgen05 GEMM instead of `dequant` + `F.linear` (:231-275);
+  dequant->wgmma GEMM instead of `dequant` + `F.linear` (:231-275);
 * `argsort(perm)` is not recomputed on every call (the reference does, :208-211).
 """
 from __future__ import annotations

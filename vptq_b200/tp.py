@@ -5,7 +5,7 @@ BASELINE.json's north_star: rank p owns index rows [p*Ro/P, (p+1)*Ro/P) -- whole
 packed index tensor, so the wire format is untouched -- plus the matching slices of
 `outlier_indices` and `bias`; codebooks, `perm`, `weight_scale`, `weight_bias` are indexed by
 input column and are replicated.  Each rank computes its slice of y with the fused GEMV /
-tcgen05 GEMM and ONE collective per layer completes y on every rank:
+wgmma GEMM and ONE collective per layer completes y on every rank:
 
     mode "all_reduce" (north_star): write the slice into a zeroed full-width y, NCCL all-reduce(sum)
     mode "all_gather":              NCCL all-gather of the slices (same result, 1/P of the bytes)
