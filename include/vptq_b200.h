@@ -43,7 +43,7 @@
 extern "C" {
 #endif
 
-#define VPTQ_B200_ABI_VERSION 6
+#define VPTQ_B200_ABI_VERSION 7
 
 #if defined(__GNUC__)
 #define VPTQ_B200_API __attribute__((visibility("default")))
@@ -70,6 +70,11 @@ typedef enum vptq_status {
                             weights/codebooks/indices before griddepcontrol.wait and only then
                             reads x; legal whenever x is produced by the preceding kernel on
                             the same stream */
+#define VPTQ_FLAG_TRANSPOSE 2u /* vptq_b200_quant_gemm only: compute the layer's INPUT GRADIENT
+                                  y[tokens][in_features] = x[tokens][out_features] . W instead of
+                                  x W^T + bias (bias is not applied; x_stride >= out_features,
+                                  y_stride >= in_features).  Workspace: VPTQ_OP_GEMM_DGRAD.  Any
+                                  tokens >= 1.  Libraries before ABI 7 ignore this flag. */
 
 /*
  * One VQuantLinear layer: exactly the tensors the reference module owns
@@ -147,7 +152,8 @@ typedef enum vptq_op {
   VPTQ_OP_GEMV = 0,    /* vptq_b200_quant_gemv    */
   VPTQ_OP_DEQUANT = 1, /* vptq_b200_dequant       */
   VPTQ_OP_GEMM = 2,    /* vptq_b200_quant_gemm    */
-  VPTQ_OP_GEMV_V2 = 3  /* vptq_b200_quant_gemv_v2 */
+  VPTQ_OP_GEMV_V2 = 3, /* vptq_b200_quant_gemv_v2 */
+  VPTQ_OP_GEMM_DGRAD = 4 /* vptq_b200_quant_gemm with VPTQ_FLAG_TRANSPOSE */
 } vptq_op;
 
 /* Developer aid (not needed by any caller): when given a device buffer of 32 uint64, every GEMV
@@ -293,6 +299,10 @@ VPTQ_B200_API int vptq_b200_dequant(const vptq_linear_desc* desc, void* w_out, v
  * vptq/ops/quant_gemm.py:231-275): the quantised weight is dequantised once into the workspace (16-bit,
  * quantised column order, scale / bias / perm kept out of it) and fed by TMA to a wgmma tensor-core
  * GEMM with register accumulators.
+ * With VPTQ_FLAG_TRANSPOSE: the input gradient dX = dY . W of the layer (x = dY [tokens][out_features],
+ * y = dX [tokens][in_features], no bias) through a transposed dequant W^T[in][out] in the workspace (original
+ * feature order, scale / bias folded in, bit-identical to the transpose of vptq_b200_dequant's W) and the same
+ * GEMM.  Gradients of the codebooks, scale and bias vectors are not computed.
  */
 VPTQ_B200_API int vptq_b200_quant_gemm(const vptq_linear_desc* desc, const void* x, int64_t x_stride, void* y,
                          int64_t y_stride, int32_t tokens, void* workspace,

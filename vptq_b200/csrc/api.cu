@@ -48,6 +48,17 @@ namespace {
 
 bool is_pow2(int64_t v) { return v > 0 && (v & (v - 1)) == 0; }
 
+int check_device() {
+  const DeviceInfo* dev = device_info();
+  if (!dev) return VPTQ_ERR_CUDA;
+  if (dev->cc_major != 9 || dev->cc_minor != 0) {
+    set_error("device compute capability %d.%d: this library contains sm_90a code only", dev->cc_major,
+              dev->cc_minor);
+    return VPTQ_ERR_DEVICE;
+  }
+  return 0;
+}
+
 // Mirrors the reference's argument checks (csrc/quant_gemv.cu:252-282, csrc/dequant.cu:238-275,
 // vptq/layers/vqlinear.py:77-81,128-146) as explicit return codes.
 int validate(const vptq_linear_desc* d, bool need_device) {
@@ -134,16 +145,7 @@ int validate(const vptq_linear_desc* d, bool need_device) {
     set_error("centroids must be 16-byte aligned (per codebook), indices 4-byte aligned");
     return VPTQ_ERR_INVALID;
   }
-  if (need_device) {
-    const DeviceInfo* dev = device_info();
-    if (!dev) return VPTQ_ERR_CUDA;
-    if (dev->cc_major != 9 || dev->cc_minor != 0) {
-      set_error("device compute capability %d.%d: this library contains sm_90a code only", dev->cc_major,
-                dev->cc_minor);
-      return VPTQ_ERR_DEVICE;
-    }
-  }
-  return 0;
+  return need_device ? check_device() : 0;
 }
 
 int need_packed(const vptq_linear_desc* d, const char* what) {
@@ -181,6 +183,7 @@ size_t vptq_b200_workspace_bytes(const vptq_linear_desc* desc, int32_t tokens, i
     }
     case VPTQ_OP_DEQUANT: return dequant_workspace_bytes(*desc);
     case VPTQ_OP_GEMM: return gemm_workspace_bytes(*desc, tokens);
+    case VPTQ_OP_GEMM_DGRAD: return dgrad_workspace_bytes(*desc, tokens);
     default: set_error("workspace_bytes: unknown op %d", op); return 0;
   }
 }
@@ -286,6 +289,19 @@ int vptq_b200_dequant(const vptq_linear_desc* desc, void* w_out, void* workspace
 int vptq_b200_quant_gemm(const vptq_linear_desc* desc, const void* x, int64_t x_stride, void* y,
                          int64_t y_stride, int32_t tokens, void* workspace, size_t workspace_bytes,
                          uint32_t flags, void* stream) {
+  if (flags & VPTQ_FLAG_TRANSPOSE) {  // input gradient: x = dY [tokens][O], y = dX [tokens][I]
+    if (int rc = validate(desc, false)) return rc;
+    if (!x || !y || tokens < 1 || x_stride < desc->out_features || y_stride < desc->in_features) {
+      set_error("quant_gemm (transpose): bad x/y/tokens/strides (x_stride %lld must be >= out_features %d, y_stride "
+                "%lld >= in_features %d)", (long long)x_stride, desc->out_features, (long long)y_stride,
+                desc->in_features);
+      return VPTQ_ERR_INVALID;
+    }
+    if (int rc = need_packed(desc, "quant_gemm (transpose)")) return rc;
+    if (int rc = check_device()) return rc;
+    return dgrad_launch(*desc, x, x_stride, y, y_stride, tokens, workspace, workspace_bytes,
+                        static_cast<cudaStream_t>(stream));
+  }
   if (int rc = validate(desc, true)) return rc;
   if (!x || !y || tokens < 1 || x_stride < desc->in_features || y_stride < desc->out_features) {
     set_error("quant_gemm: bad x/y/tokens/strides");

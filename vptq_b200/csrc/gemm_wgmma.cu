@@ -19,6 +19,9 @@
 //                         in registers (m64n256k16, 128 registers per thread); its epilogue (adds
 //                         rowbias[t] + bias[o], writes 16-bit y) runs while the producer already fills the
 //                         ring with the next tile's operands.
+//
+// The same GEMM computes the layer's input gradient dX = dY . W (VPTQ_FLAG_TRANSPOSE, dgrad_launch below) from a
+// TRANSPOSED dequant Wt[I][O] (dequant.cu): A = dY, B = Wt, N = in_features, K = out_features.
 #include <cuda.h>
 
 #include <algorithm>
@@ -33,7 +36,6 @@ namespace vptq_b200 {
 
 // implemented in dequant.cu
 int dequant_quant_order_launch(const vptq_linear_desc& d, void* wq_out, int64_t ld, cudaStream_t stream);
-
 namespace {
 
 constexpr int BM = 128, BN = 256, BK = 64;  // CTA tile: tokens x outputs x reduction
@@ -397,9 +399,81 @@ GemmWorkspace gemm_layout(const vptq_linear_desc& d, int tokens) {
   return w;
 }
 
+// Input gradient dX[T][I] = dY[T][O] . W: the same GEMM with A = dY, B = Wt[I][ld] (transposed dequant, K = ld
+// = O rounded up to whole BK blocks, its columns [O, ld) zero).  dY goes to TMA as it is when its rows are
+// 16-byte aligned whole BK blocks; otherwise it is first copied to [T][ld] with zero K padding.
+struct DgradWorkspace {
+  size_t off_wt, off_dy, total;
+  int64_t ld;
+};
+DgradWorkspace dgrad_layout(const vptq_linear_desc& d, int tokens) {
+  DgradWorkspace w;
+  w.ld = int64_t(align_up(size_t(d.out_features), 64));
+  size_t off = kZeroRegionBytes;                         // the zero-at-rest region stays untouched
+  w.off_wt = off;
+  off += align_up(size_t(d.in_features) * w.ld * 2, 1024);
+  w.off_dy = off;
+  off += align_up(size_t(tokens) * w.ld * 2, 1024);
+  w.total = off;
+  return w;
+}
+
+// dy rows -> pitch ld, columns [O, ld) <- 0 (16-bit payload copied as it is)
+__global__ void dgrad_stage_dy(const uint16_t* __restrict__ dy, int64_t dy_stride, uint16_t* __restrict__ out,
+                               int64_t ld, int O) {
+  const uint16_t* src = dy + int64_t(blockIdx.x) * dy_stride;
+  uint16_t* dst = out + int64_t(blockIdx.x) * ld;
+  for (int64_t c = threadIdx.x; c < ld; c += blockDim.x) dst[c] = c < O ? src[c] : uint16_t(0);
+}
+
 }  // namespace
 
 size_t gemm_workspace_bytes(const vptq_linear_desc& d, int tokens) { return gemm_layout(d, tokens).total; }
+
+size_t dgrad_workspace_bytes(const vptq_linear_desc& d, int tokens) { return dgrad_layout(d, tokens).total; }
+
+int dgrad_launch(const vptq_linear_desc& d, const void* dy, int64_t dy_stride, void* dx, int64_t dx_stride, int tokens,
+                 void* workspace, size_t workspace_bytes, cudaStream_t stream) {
+  const DgradWorkspace w = dgrad_layout(d, tokens);
+  if (!workspace || workspace_bytes < w.total) {
+    set_error("quant_gemm (transpose): workspace %zu bytes < required %zu", workspace_bytes, w.total);
+    return VPTQ_ERR_WORKSPACE;
+  }
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  void* wt = ws + w.off_wt;
+  const int is_bf16 = d.dtype == VPTQ_BF16;
+  if (int rc = dequant_transposed_launch(d, wt, w.ld, stream)) return rc;
+  const void* a = dy;
+  int64_t a_ld = dy_stride;
+  if (int64_t(d.out_features) != w.ld || (reinterpret_cast<uintptr_t>(dy) & 15u) || (dy_stride % 8)) {
+    a = ws + w.off_dy, a_ld = w.ld;
+    dgrad_stage_dy<<<tokens, 256, 0, stream>>>(reinterpret_cast<const uint16_t*>(dy), dy_stride,
+                                                reinterpret_cast<uint16_t*>(ws + w.off_dy), w.ld, d.out_features);
+  }
+  CUtensorMap map_a, map_b;
+  if (int rc = make_map(&map_a, is_bf16, a, tokens, w.ld, a_ld, BM)) return rc;
+  if (int rc = make_map(&map_b, is_bf16, wt, d.in_features, w.ld, w.ld, BN)) return rc;
+  GemmParams p{};
+  p.bias = nullptr, p.rowbias = nullptr, p.y = dx, p.y_stride = dx_stride;
+  p.T = tokens, p.O = d.in_features, p.K = int(w.ld), p.is_bf16 = is_bf16;
+  const DeviceInfo* dev = device_info();
+  if (!dev) return VPTQ_ERR_CUDA;
+  const int ntiles = ((d.in_features + BN - 1) / BN) * ((tokens + BM - 1) / BM);
+  dim3 grid(unsigned(std::min(ntiles, dev->sm_count)));  // persistent: one CTA per SM
+  if (is_bf16) {
+    if (int rc = ensure_smem_attr(reinterpret_cast<const void*>(gemm_tn_wgmma<__nv_bfloat16>), GEMM_SMEM)) return rc;
+    gemm_tn_wgmma<__nv_bfloat16><<<grid, GEMM_THREADS, GEMM_SMEM, stream>>>(map_a, map_b, p);
+  } else {
+    if (int rc = ensure_smem_attr(reinterpret_cast<const void*>(gemm_tn_wgmma<__half>), GEMM_SMEM)) return rc;
+    gemm_tn_wgmma<__half><<<grid, GEMM_THREADS, GEMM_SMEM, stream>>>(map_a, map_b, p);
+  }
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("quant_gemm (transpose) launch: %s", cudaGetErrorString(e));
+    return VPTQ_ERR_CUDA;
+  }
+  return 0;
+}
 
 int gemm_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void* y, int64_t y_stride, int tokens,
                 void* workspace, size_t workspace_bytes, uint32_t /*flags*/, cudaStream_t stream) {

@@ -112,6 +112,8 @@ size_t dequant_workspace_bytes(const vptq_linear_desc& d);
 int dequant_launch(const vptq_linear_desc& d, void* w_out, void* workspace, size_t workspace_bytes,
                    cudaStream_t stream, int64_t ld = 0);
 bool dequant_orig_fast_ok(const vptq_linear_desc& d, const void* w_out, int64_t ld);  // 8-columns-per-thread path applies
+// Wt[f][o] = W[o][f], rows in original feature order, pitch ld (multiple of 8, >= out_features), columns [O, ld) zero
+int dequant_transposed_launch(const vptq_linear_desc& d, void* wt_out, int64_t ld, cudaStream_t stream);
 
 // -------------------------------------------------------------------------------------------
 // prefill GEMM (wgmma)
@@ -119,6 +121,10 @@ bool dequant_orig_fast_ok(const vptq_linear_desc& d, const void* w_out, int64_t 
 size_t gemm_workspace_bytes(const vptq_linear_desc& d, int tokens);
 int gemm_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void* y, int64_t y_stride,
                 int tokens, void* workspace, size_t workspace_bytes, uint32_t flags, cudaStream_t stream);
+// input gradient dx[T][I] = dy[T][O] . W (no bias): transposed dequant + the same wgmma GEMM
+size_t dgrad_workspace_bytes(const vptq_linear_desc& d, int tokens);
+int dgrad_launch(const vptq_linear_desc& d, const void* dy, int64_t dy_stride, void* dx, int64_t dx_stride, int tokens,
+                 void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 // -------------------------------------------------------------------------------------------
 // v2 GEMV (unpacked indices)

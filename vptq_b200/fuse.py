@@ -57,6 +57,8 @@ class FusedGroup:
 
         The cached outputs are handed to every member at most once: an address + version match alone could be a
         NEW tensor the caching allocator placed where the previous activation lived."""
+        if torch.is_grad_enabled() and x.requires_grad:
+            return None           # the member's own forward records the autograd graph (same values)
         x2 = x.reshape(-1, x.shape[-1])
         tokens = x2.shape[0]
         if not x.is_cuda or tokens < 1 or tokens > 2 or x2.stride(-1) != 1:

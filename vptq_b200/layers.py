@@ -37,6 +37,14 @@ def _frozen(shape, dtype, device) -> Parameter:
 
 
 class VQuantLinear(nn.Module):
+    """VPTQ quantized linear layer (see the module docstring for the tensors it holds).
+
+    Autograd: when grad mode is on and `x.requires_grad`, `forward` records a backward that gives `x` its gradient
+    (dX = dY W: a transposed dequant feeding the wgmma GEMM) and `bias` its gradient -- what adapters (LoRA / PEFT)
+    trained on top of a frozen quantized model need.  The codebooks, `weight_scale` and `weight_bias` get no
+    gradient: `set_centroids_grad` has no effect on this path, as with the reference's CUDA extension.  There is no
+    double backward, and the backward of a decode-only module (`prepare(drop_packed=True)`) raises."""
+
     def __init__(
         self,
         in_features: int,
@@ -257,6 +265,7 @@ class VQuantLinear(nn.Module):
         return diff.T @ diff * H
 
     def set_centroids_grad(self, requires_grad: bool) -> None:
+        """Sets `requires_grad` on the codebooks (reference surface); the CUDA path computes no codebook gradient."""
         self.centroids.weight.requires_grad = requires_grad
         if self.enable_outlier:
             self.outlier_centroids.weight.requires_grad = requires_grad

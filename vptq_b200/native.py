@@ -20,10 +20,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("VPTQ_B200_LIB") or os.path.join(_HERE, "libvptq_b200.so")   # (env: developer builds)
 
 VPTQ_FP16, VPTQ_BF16 = 0, 1
-OP_GEMV, OP_DEQUANT, OP_GEMM, OP_GEMV_V2 = 0, 1, 2, 3
-FLAG_PDL = 1
+OP_GEMV, OP_DEQUANT, OP_GEMM, OP_GEMV_V2, OP_GEMM_DGRAD = 0, 1, 2, 3, 4
+FLAG_PDL, FLAG_TRANSPOSE = 1, 2
 TP_PLAIN, TP_TAGGED = 0, 1
-ABI_VERSION = 6
+ABI_VERSION = 7
 LISTS_DEFAULT = "1"   # VPTQ_B200_LISTS when unset
 
 EXPORTS = (
@@ -364,6 +364,21 @@ def quant_gemm(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, flags: in
         rc = lib().vptq_b200_quant_gemm(ctypes.byref(desc), x2d.data_ptr(), x2d.stride(0), y2d.data_ptr(),
                                         y2d.stride(0), tokens, ws.data_ptr(), ws.numel(), flags, _stream(dev))
     check(rc, "vptq_b200_quant_gemm")
+
+
+def quant_gemm_dgrad(desc: LinearDesc, dy2d: torch.Tensor, dx2d: torch.Tensor) -> None:
+    """dx2d [tokens, in_features] = dy2d [tokens, out_features] @ W: the layer's input gradient
+    (vptq_b200_quant_gemm with VPTQ_FLAG_TRANSPOSE).  Any token count."""
+    tokens = dy2d.shape[0]
+    if dy2d.stride(-1) != 1 or (tokens > 1 and dy2d.stride(0) < dy2d.shape[1]):
+        dy2d = dy2d.contiguous()      # autograd hands over expanded (zero-stride) gradients, e.g. from y.sum()
+    pitch = lambda t: t.stride(0) if t.shape[0] > 1 else t.shape[1]   # (a one-row tensor may carry any row stride)
+    dev = dy2d.device
+    with _on_device(dev):
+        ws = workspace(dev, _ws_bytes_cached(desc, tokens, OP_GEMM_DGRAD))
+        rc = lib().vptq_b200_quant_gemm(ctypes.byref(desc), dy2d.data_ptr(), pitch(dy2d), dx2d.data_ptr(),
+                                        pitch(dx2d), tokens, ws.data_ptr(), ws.numel(), FLAG_TRANSPOSE, _stream(dev))
+    check(rc, "vptq_b200_quant_gemm (transpose)")
 
 
 def dequant(desc: LinearDesc, w_out: torch.Tensor) -> None:

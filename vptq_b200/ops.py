@@ -15,6 +15,7 @@ from __future__ import annotations
 from typing import Optional
 
 import torch
+from torch.autograd.function import once_differentiable
 
 from . import native
 
@@ -149,15 +150,59 @@ def quant_gemm(
     x2d = x.reshape(-1, in_features)
     if x2d.stride(-1) != 1:
         x2d = x2d.contiguous()
-    tokens = x2d.shape[0]
-    y = torch.empty(tokens, out_features, dtype=x.dtype, device=x.device)
-    if tokens == 0:
+    if torch.is_grad_enabled() and x.requires_grad:
+        # keeps the descriptor (and the uint16 perm it points to) alive until backward, also for a one-off descriptor
+        keep = _desc_cache[:2] if _desc_cache is not None else [desc, perm_]
+        layer = (indices, centroids, residual_centroids, outlier_indices, outlier_centroids, perm, weight_scale,
+                 weight_bias)
+        y = _QuantLinearFn.apply(x2d, bias, keep, out_features, *[t for t in layer if t is not None])
         return y.reshape(*x.shape[:-1], out_features)
+    return _forward(desc, x2d, out_features).reshape(*x.shape[:-1], out_features)
+
+
+def _forward(desc, x2d: torch.Tensor, out_features: int) -> torch.Tensor:
+    tokens = x2d.shape[0]
+    y = torch.empty(tokens, out_features, dtype=x2d.dtype, device=x2d.device)
+    if tokens == 0:
+        return y
     if tokens < 3:
         native.quant_gemv(desc, x2d, y)
     else:
         native.quant_gemm(desc, x2d, y)
-    return y.reshape(*x.shape[:-1], out_features)
+    return y
+
+
+class _QuantLinearFn(torch.autograd.Function):
+    """y = x W^T + bias with gradients for x and bias.
+
+    forward: the no-grad routing above, so values are bit-identical to a call under torch.no_grad().
+    backward: dX = dY W through the transposed dequant + wgmma GEMM (vptq_b200_quant_gemm with VPTQ_FLAG_TRANSPOSE)
+    for any token count; dbias = dY summed over tokens in fp32.  The codebooks, weight_scale and weight_bias get no
+    gradient (the reference's CUDA path does not give them one either).  The layer tensors are saved so that an
+    in-place update between forward and backward fails autograd's version check instead of using new weights."""
+
+    @staticmethod
+    def forward(ctx, x2d, bias, keep, out_features, *layer):
+        ctx.keep = keep
+        ctx.save_for_backward(*layer)
+        return _forward(keep[0], x2d, out_features)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        ctx.saved_tensors            # version check of the layer tensors
+        desc = ctx.keep[0]
+        if not desc.indices:
+            raise RuntimeError("backward through a decode-only VQuantLinear (prepare(drop_packed=True)): the input "
+                               "gradient needs the packed index words, which were freed; reload the checkpoint")
+        dx = dbias = None
+        if ctx.needs_input_grad[0]:
+            dx = torch.empty(dy.shape[0], desc.in_features, dtype=dy.dtype, device=dy.device)
+            if dy.shape[0]:
+                native.quant_gemm_dgrad(desc, dy, dx)
+        if ctx.needs_input_grad[1]:
+            dbias = dy.float().sum(0).to(dy.dtype)
+        return (dx, dbias, None, None) + (None,) * len(ctx.saved_tensors)
 
 
 def quant_gemv_v2(
