@@ -61,7 +61,7 @@ class FusedGroup:
             return None           # the member's own forward records the autograd graph (same values)
         x2 = x.reshape(-1, x.shape[-1])
         tokens = x2.shape[0]
-        if not x.is_cuda or tokens < 1 or tokens > 2 or x2.stride(-1) != 1:
+        if not x.is_cuda or tokens < 1 or tokens > 2 or x2.stride(-1) != 1 or (tokens > 1 and x2.stride(0) < x2.shape[1]):
             return None
         key = (x.data_ptr(), x._version, tuple(x.shape), x.dtype, x.device)
         if key == self._key and self._out is not None and not (self._served >> index) & 1:

@@ -281,13 +281,18 @@ def _ws_bytes_cached(desc: LinearDesc, tokens: int, op: int) -> int:
     return v
 
 
+def row_pitch(t: torch.Tensor) -> int:
+    """Row pitch in elements for the C ABI: a one-row tensor may carry any row stride (0 after `expand`)."""
+    return t.stride(0) if t.shape[0] > 1 else t.shape[1]
+
+
 def quant_gemv(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, flags: int = 0) -> None:
     dev = x2d.device
     tokens = x2d.shape[0]
     with _on_device(dev):
         ws = workspace(dev, _ws_bytes_cached(desc, tokens, OP_GEMV))
-        rc = lib().vptq_b200_quant_gemv(ctypes.byref(desc), x2d.data_ptr(), x2d.stride(0), y2d.data_ptr(),
-                                        y2d.stride(0), tokens, ws.data_ptr(), ws.numel(), flags, _stream(dev))
+        rc = lib().vptq_b200_quant_gemv(ctypes.byref(desc), x2d.data_ptr(), row_pitch(x2d), y2d.data_ptr(),
+                                        row_pitch(y2d), tokens, ws.data_ptr(), ws.numel(), flags, _stream(dev))
     check(rc, "vptq_b200_quant_gemv")
 
 
@@ -314,7 +319,7 @@ class FusedGemv:
                 if self.ws_bytes is None:
                     self.ws_bytes = sum(workspace_bytes(d, x2d.shape[0], OP_GEMV) for d in self.descs)
                 ws = workspace(dev, self.ws_bytes)   # the list kernel reduces its partial sums through it
-                rc = lib().vptq_b200_quant_gemv_multi_ws(self.n, self.desc_arr, x2d.data_ptr(), x2d.stride(0),
+                rc = lib().vptq_b200_quant_gemv_multi_ws(self.n, self.desc_arr, x2d.data_ptr(), row_pitch(x2d),
                                                          self.y_arr, self.stride_arr, x2d.shape[0], ws.data_ptr(),
                                                          ws.numel(), flags, _stream(dev))
             if rc != -2:                      # VPTQ_ERR_UNSUPPORTED: these layers cannot share one launch
@@ -361,8 +366,8 @@ def quant_gemm(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, flags: in
     tokens = x2d.shape[0]
     with _on_device(dev):
         ws = workspace(dev, _ws_bytes_cached(desc, tokens, OP_GEMM))
-        rc = lib().vptq_b200_quant_gemm(ctypes.byref(desc), x2d.data_ptr(), x2d.stride(0), y2d.data_ptr(),
-                                        y2d.stride(0), tokens, ws.data_ptr(), ws.numel(), flags, _stream(dev))
+        rc = lib().vptq_b200_quant_gemm(ctypes.byref(desc), x2d.data_ptr(), row_pitch(x2d), y2d.data_ptr(),
+                                        row_pitch(y2d), tokens, ws.data_ptr(), ws.numel(), flags, _stream(dev))
     check(rc, "vptq_b200_quant_gemm")
 
 
@@ -372,12 +377,11 @@ def quant_gemm_dgrad(desc: LinearDesc, dy2d: torch.Tensor, dx2d: torch.Tensor) -
     tokens = dy2d.shape[0]
     if dy2d.stride(-1) != 1 or (tokens > 1 and dy2d.stride(0) < dy2d.shape[1]):
         dy2d = dy2d.contiguous()      # autograd hands over expanded (zero-stride) gradients, e.g. from y.sum()
-    pitch = lambda t: t.stride(0) if t.shape[0] > 1 else t.shape[1]   # (a one-row tensor may carry any row stride)
     dev = dy2d.device
     with _on_device(dev):
         ws = workspace(dev, _ws_bytes_cached(desc, tokens, OP_GEMM_DGRAD))
-        rc = lib().vptq_b200_quant_gemm(ctypes.byref(desc), dy2d.data_ptr(), pitch(dy2d), dx2d.data_ptr(),
-                                        pitch(dx2d), tokens, ws.data_ptr(), ws.numel(), FLAG_TRANSPOSE, _stream(dev))
+        rc = lib().vptq_b200_quant_gemm(ctypes.byref(desc), dy2d.data_ptr(), row_pitch(dy2d), dx2d.data_ptr(),
+                                        row_pitch(dx2d), tokens, ws.data_ptr(), ws.numel(), FLAG_TRANSPOSE, _stream(dev))
     check(rc, "vptq_b200_quant_gemm (transpose)")
 
 

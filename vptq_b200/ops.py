@@ -148,8 +148,8 @@ def quant_gemm(
         if _desc_cache is not None:
             _desc_cache.extend([desc, perm_])   # keep the converted perm alive with the descriptor
     x2d = x.reshape(-1, in_features)
-    if x2d.stride(-1) != 1:
-        x2d = x2d.contiguous()
+    if x2d.stride(-1) != 1 or (x2d.shape[0] > 1 and x2d.stride(0) < in_features):
+        x2d = x2d.contiguous()    # broadcast rows (expand, overlapping unfold windows): the kernels need pitch >= I
     if torch.is_grad_enabled() and x.requires_grad:
         # keeps the descriptor (and the uint16 perm it points to) alive until backward, also for a one-off descriptor
         keep = _desc_cache[:2] if _desc_cache is not None else [desc, perm_]
