@@ -302,7 +302,7 @@ VPTQ_B200_API int vptq_b200_dequant(const vptq_linear_desc* desc, void* w_out, v
  * With VPTQ_FLAG_TRANSPOSE: the input gradient dX = dY . W of the layer (x = dY [tokens][out_features],
  * y = dX [tokens][in_features], no bias) through a transposed dequant W^T[in][out] in the workspace (original
  * feature order, scale / bias folded in, bit-identical to the transpose of vptq_b200_dequant's W) and the same
- * GEMM.  Gradients of the codebooks, scale and bias vectors are not computed.
+ * GEMM.  Gradients of the codebooks, scale and bias vectors: include/vptq_b200_grad.h.
  */
 VPTQ_B200_API int vptq_b200_quant_gemm(const vptq_linear_desc* desc, const void* x, int64_t x_stride, void* y,
                          int64_t y_stride, int32_t tokens, void* workspace,

@@ -154,6 +154,31 @@ int need_packed(const vptq_linear_desc* d, const char* what) {
   return VPTQ_ERR_UNSUPPORTED;
 }
 
+// the gradient outputs must match tensors the layer has, 16-bit aligned
+int validate_grads(const vptq_linear_desc* d, const vptq_linear_grads* g, uint32_t flags, uint32_t allowed_flags,
+                   const char* what) {
+  if (!g || g->struct_size != sizeof(vptq_linear_grads) || g->reserved != 0) {
+    set_error("%s: grads is NULL or its struct_size / reserved field is wrong (ABI mismatch)", what);
+    return VPTQ_ERR_INVALID;
+  }
+  if (flags & ~allowed_flags) {
+    set_error("%s: unknown flags 0x%x", what, flags);
+    return VPTQ_ERR_INVALID;
+  }
+  const bool outl = d->outlier_size > 0 && d->outlier_indices != nullptr;
+  if ((g->res_centroids && d->num_res_centroids <= 0) || (g->outlier_centroids && !outl) ||
+      ((g->weight_scale || g->weight_bias) && !d->weight_scale)) {
+    set_error("%s: a gradient was requested for a tensor this layer does not have", what);
+    return VPTQ_ERR_INVALID;
+  }
+  for (const void* p : {g->centroids, g->res_centroids, g->outlier_centroids, g->weight_scale, g->weight_bias})
+    if (reinterpret_cast<uintptr_t>(p) & 1u) {
+      set_error("%s: gradient outputs must be 2-byte aligned", what);
+      return VPTQ_ERR_INVALID;
+    }
+  return 0;
+}
+
 }  // namespace
 }  // namespace vptq_b200
 
@@ -310,6 +335,52 @@ int vptq_b200_quant_gemm(const vptq_linear_desc* desc, const void* x, int64_t x_
   if (int rc = need_packed(desc, "quant_gemm")) return rc;
   return gemm_launch(*desc, x, x_stride, y, y_stride, tokens, workspace, workspace_bytes, flags,
                      static_cast<cudaStream_t>(stream));
+}
+
+// ---- training entry points (include/vptq_b200_grad.h) ----
+int vptq_b200_grad_version(void) { return VPTQ_B200_GRAD_VERSION; }
+
+size_t vptq_b200_grad_workspace_bytes(const vptq_linear_desc* desc, int32_t tokens, int32_t op) {
+  if (validate(desc, false)) return 0;
+  if (op != VPTQ_GRAD_OP_WGRAD && op != VPTQ_GRAD_OP_DEQUANT_BACKWARD && op != VPTQ_GRAD_OP_WGRAD_GENERIC) {
+    set_error("grad_workspace_bytes: unknown op %d", op);
+    return 0;
+  }
+  return wgrad_workspace_bytes(*desc, tokens, op);
+}
+
+int vptq_b200_quant_gemm_wgrad(const vptq_linear_desc* desc, const void* x, int64_t x_stride, const void* dy,
+                               int64_t dy_stride, int32_t tokens, const vptq_linear_grads* grads, void* workspace,
+                               size_t workspace_bytes, uint32_t flags, void* stream) {
+  if (int rc = validate(desc, false)) return rc;
+  if (!x || !dy || tokens < 1 || x_stride < desc->in_features || dy_stride < desc->out_features ||
+      (reinterpret_cast<uintptr_t>(x) & 1u) || (reinterpret_cast<uintptr_t>(dy) & 1u)) {
+    set_error("quant_gemm_wgrad: bad x/dy/tokens/strides (tokens %d, x_stride %lld must be >= in_features %d, "
+              "dy_stride %lld >= out_features %d)", tokens, (long long)x_stride, desc->in_features,
+              (long long)dy_stride, desc->out_features);
+    return VPTQ_ERR_INVALID;
+  }
+  if (int rc = validate_grads(desc, grads, flags, VPTQ_GRAD_FLAG_GENERIC, "quant_gemm_wgrad")) return rc;
+  if (int rc = need_packed(desc, "quant_gemm_wgrad")) return rc;
+  if (int rc = check_device()) return rc;
+  return wgrad_launch(*desc, x, x_stride, dy, dy_stride, tokens, *grads, workspace, workspace_bytes, flags,
+                      static_cast<cudaStream_t>(stream));
+}
+
+int vptq_b200_dequant_backward(const vptq_linear_desc* desc, const void* dw, int64_t dw_stride,
+                               const vptq_linear_grads* grads, void* workspace, size_t workspace_bytes, uint32_t flags,
+                               void* stream) {
+  if (int rc = validate(desc, false)) return rc;
+  if (!dw || dw_stride < desc->in_features || (reinterpret_cast<uintptr_t>(dw) & 1u)) {
+    set_error("dequant_backward: bad dw / stride (dw_stride %lld must be >= in_features %d)", (long long)dw_stride,
+              desc->in_features);
+    return VPTQ_ERR_INVALID;
+  }
+  if (int rc = validate_grads(desc, grads, flags, 0u, "dequant_backward")) return rc;
+  if (int rc = need_packed(desc, "dequant_backward")) return rc;
+  if (int rc = check_device()) return rc;
+  return dequant_backward_launch(*desc, dw, dw_stride, *grads, workspace, workspace_bytes,
+                                 static_cast<cudaStream_t>(stream));
 }
 
 int vptq_b200_quant_gemv_v2(int32_t dtype, const void* x, void* y, int32_t tokens, int32_t in_features,

@@ -221,6 +221,10 @@ __device__ __forceinline__ void cluster_arrive_relaxed() {
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
 __device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 
+// v in units of 2^e (inv_unit = 2^-e), rounded to the nearest integer: one term of a 64-bit fixed-point sum
+// (weight gradients, wgrad.cu).  Integer addition is associative: the sum does not depend on the order.
+__device__ __forceinline__ long long to_fixed(double v, double inv_unit) { return __double2ll_rn(v * inv_unit); }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -21,7 +21,8 @@
 //                         ring with the next tile's operands.
 //
 // The same GEMM computes the layer's input gradient dX = dY . W (VPTQ_FLAG_TRANSPOSE, dgrad_launch below) from a
-// TRANSPOSED dequant Wt[I][O] (dequant.cu): A = dY, B = Wt, N = in_features, K = out_features.
+// TRANSPOSED dequant Wt[I][O] (dequant.cu): A = dY, B = Wt, N = in_features, K = out_features.  With an fp32
+// epilogue (wgrad_gamma_launch) it forms the weight-gradient product G = dY^T x for wgrad.cu.
 #include <cuda.h>
 
 #include <algorithm>
@@ -230,10 +231,92 @@ struct GemmParams {
   int is_bf16;
 };
 
+struct GemmParamsWgrad : GemmParams {
+  WgradEpilogue w;
+};
+
+// per-CTA dR table of the fused weight-gradient epilogue: behind the ring and the barriers
+constexpr int WG_TABLE_OFF = STAGES * (TILE_A_BYTES + TILE_B_BYTES) + 256;
+
+// Fused weight-gradient epilogue (EPI_WGRAD): this thread's 128 accumulators are G[o][c] for rows o = r0, r1 = r0 + 8
+// and columns c = n0 + 8j + 2(lane % 4) + {0, 1}.  With v = 8, o = 8 r + e: r0 and r1 lie in consecutive index rows
+// with the same e.  Every element adds s_c G to dC[k][e] (red.global.add.u64) and to the shared dR table; the
+// fixed-point terms of d weight_scale / d weight_bias of a column are summed over the 8 lanes that hold it
+// (shuffles; integers, so the order is irrelevant) and added once per warp.
 template <typename T>
+__device__ __forceinline__ void wgrad_epilogue(const float (&acc)[128], const WgradEpilogue& w, const WgHeader& h,
+                                               unsigned long long* table, int r0, int n0, int M, int lane) {
+  const double u_cb = ldexp(1.0, -h.e_cb), u_b = ldexp(1.0, -h.e_bias), u_s = ldexp(1.0, -h.e_scale);
+  const int b = w.ib + w.rb;
+  const uint32_t fmask = b >= 32 ? 0xffffffffu : ((1u << b) - 1u), imask = (1u << w.ib) - 1u;
+  const int e = r0 & 7;
+  const bool live[2] = {r0 < M, r0 + 8 < M};
+  const uint32_t* rows[2] = {w.indices + int64_t(r0 >> 3) * w.idx_stride_r,
+                             w.indices + int64_t((r0 + 8) >> 3) * w.idx_stride_r};
+  const T* C = reinterpret_cast<const T*>(w.centroids);
+  const T* R = reinterpret_cast<const T*>(w.res_centroids);
+  const T* sq = reinterpret_cast<const T*>(w.scale_q);
+  const T* sc = reinterpret_cast<const T*>(w.scale);
+  bool bad = false;
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    long long ps[2] = {0, 0}, pb[2] = {0, 0};
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int c = n0 + 8 * j + 2 * (lane & 3) + hh;
+      if (c >= w.I) continue;
+      const double s = sq ? double(DT<T>::to_float(sq[c])) : (sc ? double(DT<T>::to_float(sc[w.perm ? w.perm[c] : c])) : 1.0);
+      const uint32_t bit = uint32_t(c) * uint32_t(b), w0 = bit >> 5, sh = bit & 31u;
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr) {
+        const float gm = acc[4 * j + 2 * rr + hh];
+        if (!live[rr] || gm == 0.f) continue;
+        if (!isfinite(gm)) {
+          bad = true;
+          continue;
+        }
+        const uint32_t lo = __ldg(rows[rr] + w0);
+        const uint32_t hi = (sh + b > 32) ? __ldg(rows[rr] + w0 + 1) : 0u;  // never reads past the row
+        const uint32_t field = __funnelshift_r(lo, hi, sh) & fmask;
+        const uint32_t k = field & imask, kr = field >> w.ib;
+        const unsigned long long q = static_cast<unsigned long long>(to_fixed(s * double(gm), u_cb));
+        if (w.acc_c) atomicAdd(&w.acc_c[size_t(k) * 8 + e], q);
+        if (w.res_table) atomicAdd(&table[kr * 8 + e], q);
+        if (w.acc_s) {
+          float wq = DT<T>::to_float(C[size_t(k) * 8 + e]);
+          if (w.rb) wq += DT<T>::to_float(R[size_t(kr) * 8 + e]);
+          ps[hh] += to_fixed(double(gm) * double(wq), u_s);
+        }
+        pb[hh] += to_fixed(double(gm), u_b);
+      }
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+#pragma unroll
+      for (int o = 4; o < 32; o <<= 1) {
+        ps[hh] += __shfl_xor_sync(0xffffffffu, ps[hh], o);
+        pb[hh] += __shfl_xor_sync(0xffffffffu, pb[hh], o);
+      }
+      const int c = n0 + 8 * j + 2 * (lane & 3) + hh;
+      if (lane < 4 && c < w.I) {
+        const int f = w.perm ? int(w.perm[c]) : c;
+        if (w.acc_s && ps[hh]) atomicAdd(&w.acc_s[f], static_cast<unsigned long long>(ps[hh]));
+        if (w.acc_b && pb[hh]) atomicAdd(&w.acc_b[f], static_cast<unsigned long long>(pb[hh]));
+      }
+    }
+  }
+  if (bad) atomicExch(&w.hdr->nonfinite, 1);
+}
+
+constexpr int EPI_STORE16 = 0, EPI_F32 = 1, EPI_WGRAD = 2;
+
+// EPI_STORE16: + rowbias + bias, 16-bit y (the forward and the input gradient).  EPI_F32: the raw fp32 accumulators
+// to (float*) y -- no bias, no rounding (G = dY^T x for the generic weight-gradient route of wgrad.cu).  EPI_WGRAD:
+// wgrad_epilogue above, nothing stored (P = GemmParamsWgrad).
+template <typename T, int EPI = EPI_STORE16, typename P = GemmParams>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tn_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-              const __grid_constant__ GemmParams p) {
+              const __grid_constant__ P p) {
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles must start on 1024-byte boundaries
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -241,6 +324,9 @@ gemm_tn_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
   uint8_t* sb = smem + STAGES * TILE_A_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + STAGES * (TILE_A_BYTES + TILE_B_BYTES));
   uint64_t* empty = full + STAGES;
+  unsigned long long* table = reinterpret_cast<unsigned long long*>(smem + WG_TABLE_OFF);
+  if constexpr (EPI == EPI_WGRAD)
+    for (int i = threadIdx.x; i < p.w.res_table; i += blockDim.x) table[i] = 0ull;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nkb = (p.K + BK - 1) / BK;
@@ -311,6 +397,24 @@ gemm_tn_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
     // accumulator layout of m64nNk16: thread (warp w, lane l) of the warpgroup holds rows 16w + l/4 and
     // 16w + l/4 + 8, columns 8j + 2(l%4) + {0, 1} for j = 0 .. N/8-1, as acc[4j .. 4j+3]
     const int r0 = m0 + wg * 64 + (wt >> 5) * 16 + (lane >> 2), r1 = r0 + 8;
+    if constexpr (EPI == EPI_WGRAD) {
+      const WgHeader h = *p.w.hdr;
+      if (!h.nonfinite) wgrad_epilogue<T>(acc, p.w, h, table, r0, n0, p.T, lane);
+      continue;
+    }
+    if constexpr (EPI == EPI_F32) {
+      float* g0 = reinterpret_cast<float*>(p.y) + int64_t(r0) * p.y_stride;
+      float* g1 = reinterpret_cast<float*>(p.y) + int64_t(r1) * p.y_stride;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + 2 * (lane & 3);
+        if (n + 1 < p.O) {   // y_stride and O even (wgrad_gamma_launch): one 8-byte store
+          if (r0 < p.T) *reinterpret_cast<float2*>(g0 + n) = make_float2(acc[4 * j], acc[4 * j + 1]);
+          if (r1 < p.T) *reinterpret_cast<float2*>(g1 + n) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+        }
+      }
+      continue;
+    }
     const float rb0 = (p.rowbias && r0 < p.T) ? p.rowbias[r0] : 0.f;
     const float rb1 = (p.rowbias && r1 < p.T) ? p.rowbias[r1] : 0.f;
     T* y0 = reinterpret_cast<T*>(p.y) + int64_t(r0) * p.y_stride;
@@ -336,6 +440,13 @@ gemm_tn_wgmma(const __grid_constant__ CUtensorMap map_a, const __grid_constant__
           }
         }
       }
+    }
+  }
+  if constexpr (EPI == EPI_WGRAD) {
+    if (p.w.res_table) {   // both consumer warpgroups are done with the table (the producer warp has returned)
+      asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS * 128) : "memory");
+      for (int i = threadIdx.x; i < p.w.res_table; i += CONSUMERS * 128)
+        if (table[i]) atomicAdd(&p.w.acc_r[i], table[i]);
     }
   }
 }
@@ -563,6 +674,72 @@ int gemm_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void
   e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_error("quant_gemm launch: %s", cudaGetErrorString(e));
+    return VPTQ_ERR_CUDA;
+  }
+  return 0;
+}
+
+int wgrad_gamma_launch(int is_bf16, const void* a, const void* b, int M, int N, int K, float* gamma, int64_t ld,
+                       cudaStream_t stream) {
+  if ((N & 1) || (ld & 1) || ld < N || (K % BK) || (reinterpret_cast<uintptr_t>(gamma) & 7u)) {
+    set_error("wgrad GEMM: N %d / ld %lld must be even, K %d a multiple of %d", N, (long long)ld, K, BK);
+    return VPTQ_ERR_INVALID;
+  }
+  CUtensorMap map_a, map_b;
+  if (int rc = make_map(&map_a, is_bf16, a, M, K, K, BM)) return rc;
+  if (int rc = make_map(&map_b, is_bf16, b, N, K, K, BN)) return rc;
+  GemmParams p{};
+  p.bias = nullptr, p.rowbias = nullptr, p.y = gamma, p.y_stride = ld;
+  p.T = M, p.O = N, p.K = K, p.is_bf16 = is_bf16;
+  const DeviceInfo* dev = device_info();
+  if (!dev) return VPTQ_ERR_CUDA;
+  const int ntiles = ((N + BN - 1) / BN) * ((M + BM - 1) / BM);
+  dim3 grid(unsigned(std::min(ntiles, dev->sm_count)));
+  if (is_bf16) {
+    if (int rc = ensure_smem_attr(reinterpret_cast<const void*>(gemm_tn_wgmma<__nv_bfloat16, EPI_F32>), GEMM_SMEM)) return rc;
+    gemm_tn_wgmma<__nv_bfloat16, EPI_F32><<<grid, GEMM_THREADS, GEMM_SMEM, stream>>>(map_a, map_b, p);
+  } else {
+    if (int rc = ensure_smem_attr(reinterpret_cast<const void*>(gemm_tn_wgmma<__half, EPI_F32>), GEMM_SMEM)) return rc;
+    gemm_tn_wgmma<__half, EPI_F32><<<grid, GEMM_THREADS, GEMM_SMEM, stream>>>(map_a, map_b, p);
+  }
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("wgrad GEMM launch: %s", cudaGetErrorString(e));
+    return VPTQ_ERR_CUDA;
+  }
+  return 0;
+}
+
+int wgrad_fused_launch(int is_bf16, const void* a, const void* b, int M, int N, int K, const WgradEpilogue& ep,
+                       cudaStream_t stream) {
+  const int smem = GEMM_SMEM + ep.res_table * 8;
+  if ((K % BK) || ep.res_table * 8 > 16 * 1024) {
+    set_error("wgrad fused GEMM: K %d must be a multiple of %d, Kr * 8 <= 2048", K, BK);
+    return VPTQ_ERR_INVALID;
+  }
+  CUtensorMap map_a, map_b;
+  if (int rc = make_map(&map_a, is_bf16, a, M, K, K, BM)) return rc;
+  if (int rc = make_map(&map_b, is_bf16, b, N, K, K, BN)) return rc;
+  GemmParamsWgrad p{};
+  p.bias = nullptr, p.rowbias = nullptr, p.y = nullptr, p.y_stride = 0;
+  p.T = M, p.O = N, p.K = K, p.is_bf16 = is_bf16;
+  p.w = ep;
+  const DeviceInfo* dev = device_info();
+  if (!dev) return VPTQ_ERR_CUDA;
+  const int ntiles = ((N + BN - 1) / BN) * ((M + BM - 1) / BM);
+  dim3 grid(unsigned(std::min(ntiles, dev->sm_count)));
+  if (is_bf16) {
+    const void* fn = reinterpret_cast<const void*>(gemm_tn_wgmma<__nv_bfloat16, EPI_WGRAD, GemmParamsWgrad>);
+    if (int rc = ensure_smem_attr(fn, GEMM_SMEM + 16 * 1024)) return rc;
+    gemm_tn_wgmma<__nv_bfloat16, EPI_WGRAD, GemmParamsWgrad><<<grid, GEMM_THREADS, smem, stream>>>(map_a, map_b, p);
+  } else {
+    const void* fn = reinterpret_cast<const void*>(gemm_tn_wgmma<__half, EPI_WGRAD, GemmParamsWgrad>);
+    if (int rc = ensure_smem_attr(fn, GEMM_SMEM + 16 * 1024)) return rc;
+    gemm_tn_wgmma<__half, EPI_WGRAD, GemmParamsWgrad><<<grid, GEMM_THREADS, smem, stream>>>(map_a, map_b, p);
+  }
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("wgrad fused GEMM launch: %s", cudaGetErrorString(e));
     return VPTQ_ERR_CUDA;
   }
   return 0;

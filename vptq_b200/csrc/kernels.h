@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include "../../include/vptq_b200.h"
+#include "../../include/vptq_b200_grad.h"
 
 namespace vptq_b200 {
 
@@ -125,6 +126,45 @@ int gemm_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void
 size_t dgrad_workspace_bytes(const vptq_linear_desc& d, int tokens);
 int dgrad_launch(const vptq_linear_desc& d, const void* dy, int64_t dy_stride, void* dx, int64_t dx_stride, int tokens,
                  void* workspace, size_t workspace_bytes, cudaStream_t stream);
+// gamma[M][ld] (fp32, unrounded) = A[M][K] . B[N][K]^T with both operands K-major, K % 64 == 0, N and ld even
+int wgrad_gamma_launch(int is_bf16, const void* a, const void* b, int M, int N, int K, float* gamma, int64_t ld,
+                       cudaStream_t stream);
+
+// Per-call state of the weight-gradient reduction (wgrad.cu), in the workspace.
+struct WgHeader {
+  int e_cb, e_bias, e_scale;       // fixed-point value q stands for q * 2^e
+  int nonfinite;                   // 1: some input value (or an fp32 element of G) was inf / NaN
+  uint32_t max_c, max_r, max_col;  // bit patterns of max |C|, |R|, |Col| (non-negative floats order like integers)
+};
+
+// Fused weight-gradient epilogue of the wgmma GEMM (G = dY^T x' with M = out_features, N = in_features in
+// quantised column order): v = 8, one codebook group, no outlier columns, Kr <= 256.  Every accumulator element
+// goes straight into the fixed-point sums; G is never stored.
+struct WgradEpilogue {
+  const uint32_t* indices;
+  int64_t idx_stride_r;
+  const void* centroids;
+  const void* res_centroids;
+  const void* scale_q;      // weight_scale in quantised column order, or nullptr (then scale[perm[c]])
+  const void* scale;        // weight_scale [I] or nullptr
+  const uint16_t* perm;     // or nullptr
+  unsigned long long *acc_c, *acc_r, *acc_s, *acc_b;  // nullptr: not wanted
+  WgHeader* hdr;
+  int I, ib, rb;
+  int res_table;            // entries of the per-CTA shared-memory dR table (Kr * 8), 0: dR not wanted
+};
+int wgrad_fused_launch(int is_bf16, const void* a, const void* b, int M, int N, int K, const WgradEpilogue& e,
+                       cudaStream_t stream);
+
+// -------------------------------------------------------------------------------------------
+// weight gradients (wgrad.cu, C interface include/vptq_b200_grad.h)
+// -------------------------------------------------------------------------------------------
+size_t wgrad_workspace_bytes(const vptq_linear_desc& d, int tokens, int op);
+int wgrad_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, const void* dy, int64_t dy_stride,
+                 int tokens, const vptq_linear_grads& g, void* workspace, size_t workspace_bytes, uint32_t flags,
+                 cudaStream_t stream);
+int dequant_backward_launch(const vptq_linear_desc& d, const void* dw, int64_t dw_stride, const vptq_linear_grads& g,
+                            void* workspace, size_t workspace_bytes, cudaStream_t stream);
 
 // -------------------------------------------------------------------------------------------
 // v2 GEMV (unpacked indices)

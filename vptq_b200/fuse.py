@@ -27,7 +27,7 @@ import torch.nn as nn
 from . import native
 from .layers import VQuantLinear
 
-__all__ = ["fuse", "unfuse", "FusedGroup", "FusedMember", "DEFAULT_GROUPS"]
+__all__ = ["fuse", "unfuse", "set_quant_grad", "FusedGroup", "FusedMember", "DEFAULT_GROUPS"]
 
 DEFAULT_GROUPS: Tuple[Tuple[str, ...], ...] = (("q_proj", "k_proj", "v_proj"), ("gate_proj", "up_proj"))
 
@@ -57,7 +57,7 @@ class FusedGroup:
 
         The cached outputs are handed to every member at most once: an address + version match alone could be a
         NEW tensor the caching allocator placed where the previous activation lived."""
-        if torch.is_grad_enabled() and x.requires_grad:
+        if torch.is_grad_enabled() and (x.requires_grad or any(l._quant_grad_needed() for l in self.layers)):
             return None           # the member's own forward records the autograd graph (same values)
         x2 = x.reshape(-1, x.shape[-1])
         tokens = x2.shape[0]
@@ -168,6 +168,19 @@ def fuse(model: nn.Module, groups: Sequence[Sequence[str]] = DEFAULT_GROUPS, pdl
             if isinstance(mod, VQuantLinear) and mod.centroids.weight.is_cuda and not mod.enable_proxy_error:
                 mod.prepare()
     return made
+
+
+def set_quant_grad(model: nn.Module, enabled: bool = True) -> int:
+    """`VQuantLinear.set_quant_grad(enabled)` on every VQuantLinear of `model`, fused members included.  Returns how
+    many layers it reached."""
+    layers = [mod.layer if isinstance(mod, FusedMember) else mod for mod in model.modules()]
+    layers = [l for l in layers if isinstance(l, VQuantLinear)]
+    if enabled:
+        for l in layers:          # refuse before any layer changes: all or nothing
+            l._check_quant_grad_possible()
+    for l in layers:
+        l.set_quant_grad(enabled)
+    return len(layers)
 
 
 def unfuse(model: nn.Module) -> int:

@@ -41,9 +41,15 @@ class VQuantLinear(nn.Module):
 
     Autograd: when grad mode is on and `x.requires_grad`, `forward` records a backward that gives `x` its gradient
     (dX = dY W: a transposed dequant feeding the wgmma GEMM) and `bias` its gradient -- what adapters (LoRA / PEFT)
-    trained on top of a frozen quantized model need.  The codebooks, `weight_scale` and `weight_bias` get no
-    gradient: `set_centroids_grad` has no effect on this path, as with the reference's CUDA extension.  There is no
-    double backward, and the backward of a decode-only module (`prepare(drop_packed=True)`) raises."""
+    trained on top of a frozen quantized model need.
+
+    Fine-tuning the quantized layer itself is opt-in: after `set_quant_grad(True)` the codebooks (`centroids`,
+    `res_centroids`, `outlier_centroids`), `weight_scale` and `weight_bias` get gradients too, through `forward`
+    (also when x does not require grad) and through `dequant()` / `proxy_error_forward`.  Their `requires_grad`
+    (see `set_centroids_grad`) decides which ones are computed; they come out in the parameter's dtype, summed in
+    64-bit fixed point and rounded once, bit-identical from run to run (include/vptq_b200_grad.h).  Without the
+    opt-in they get no gradient, as with the reference's CUDA extension.  Indices and perm never get one.  There is
+    no double backward, and the backward of a decode-only module (`prepare(drop_packed=True)`) raises."""
 
     def __init__(
         self,
@@ -146,6 +152,7 @@ class VQuantLinear(nn.Module):
         self._desc_cache: list = []      # [LinearDesc, perm16] built on first forward
         self._desc_key = None
         self._packed = None              # lazily packed indices for unpacked checkpoints
+        self._quant_grad = False         # set_quant_grad
 
     # ------------------------------------------------------------------------------------------
     def _tensors(self):
@@ -169,6 +176,53 @@ class VQuantLinear(nn.Module):
         # data_ptr catches .to() / re-assignment, _version catches in-place updates (load_state_dict, copy_)
         return tuple((a.data_ptr(), a.dtype, a._version) if a is not None else None for a in t) + (dtype, device)
 
+    # positions in _tensors() of the floating-point tensors the descriptor only points to (codebooks, scale, bias):
+    # an in-place update of them (an optimizer step) keeps the descriptor and its index lists
+    _FLOAT_SLOTS = (1, 2, 4, 6, 7, 8)
+
+    def _refresh_in_place(self, key) -> bool:
+        """Only floating-point tensors changed, in place (same storage): re-derive the quantised-order copies of
+        weight_scale / weight_bias into their buffers and keep the descriptor.  False: rebuild everything."""
+        old = self._desc_key
+        if not self._desc_cache or old is None or len(old) != len(key) or old[-2:] != key[-2:]:
+            return False
+        for i, (a, b) in enumerate(zip(old[:-2], key[:-2])):
+            if a is None or b is None:
+                if a is not b:
+                    return False
+            elif a[:2] != b[:2] or (i not in self._FLOAT_SLOTS and a[2] != b[2]):
+                return False
+        desc = self._desc_cache[0]
+        if desc._keep[:2] and desc.weight_scale_q:
+            ws_q, wb_q = desc._keep[0], desc._keep[1]
+            perm = self._desc_cache[1]
+            pidx = perm.view(torch.uint16).to(torch.int64) if perm.dtype in (torch.int16, torch.uint16) else perm.long()
+            with torch.no_grad():
+                torch.index_select(self.weight_scale, 0, pidx, out=ws_q)
+                torch.index_select(self.weight_bias, 0, pidx, out=wb_q)
+        return True
+
+    def set_quant_grad(self, enabled: bool = True) -> "VQuantLinear":
+        """Opt in to gradients for the codebooks, weight_scale and weight_bias (see the class docstring).  The
+        tensors' `requires_grad` decides which are computed.  A decode-only module refuses: its packed index words,
+        which every weight gradient reads, were freed."""
+        if enabled:
+            self._check_quant_grad_possible()
+        self._quant_grad = bool(enabled)
+        return self
+
+    def _check_quant_grad_possible(self) -> None:
+        if getattr(self, "_drop_packed", False) and self.indices.numel() == 0:
+            raise RuntimeError("set_quant_grad: this VQuantLinear is decode-only (prepare(drop_packed=True)); the "
+                               "packed index words the weight gradients need were freed; reload the checkpoint")
+
+    def _quant_grad_needed(self) -> bool:
+        """Opted in and some quantizer tensor requires grad: a forward under grad mode records a node."""
+        if not getattr(self, "_quant_grad", False):
+            return False
+        _, cent, resc, _, outc, _, ws, wb, _ = self._tensors()
+        return any(t is not None and t.requires_grad for t in (cent, resc, outc, ws, wb))
+
     def prepare(self, dtype: Optional[torch.dtype] = None, drop_packed: bool = False) -> "VQuantLinear":
         """Build the C-ABI descriptor and its load-time derivatives (scale/bias in quantised order, the
         slice x tile index lists of the decode kernel) now instead of inside the first forward: call once
@@ -182,6 +236,9 @@ class VQuantLinear(nn.Module):
         if drop_packed:
             if not self.is_indice_packed:
                 raise RuntimeError("drop_packed needs a packed checkpoint (is_indice_packed=True)")
+            if getattr(self, "_quant_grad", False):
+                raise RuntimeError("prepare(drop_packed=True) on a module with set_quant_grad(True): the weight "
+                                   "gradients need the packed index words; call set_quant_grad(False) first")
             self._desc_cache, self._desc_key = [], None
             self._drop_request = True
         try:
@@ -228,7 +285,8 @@ class VQuantLinear(nn.Module):
             else:
                 self._drop_packed = False             # a checkpoint was loaded again: a full module once more
         if key != self._desc_key:                    # parameters were moved / reloaded / updated in place
-            self._desc_cache = []
+            if not self._refresh_in_place(key):
+                self._desc_cache = []
             self._desc_key = key
         indices, cent, resc, outi, outc, perm, ws, wb, bias = t
         return ops.quant_gemm(
@@ -241,7 +299,7 @@ class VQuantLinear(nn.Module):
             outlier_size=self.outlier_size, in_features=self.in_features, out_features=self.out_features,
             padding=self.padding, outlier_padding=self.outlier_padding,
             vector_quant_dim=self.vector_quant_dim, _desc_cache=self._desc_cache,
-            _drop_packed=getattr(self, "_drop_request", False))
+            _drop_packed=getattr(self, "_drop_request", False), _quant_grad=getattr(self, "_quant_grad", False))
 
     def dequant(self) -> torch.Tensor:
         """Dense [out_features, in_features] weight through the CUDA dequant kernel."""
@@ -257,7 +315,8 @@ class VQuantLinear(nn.Module):
             num_outlier_centroids=self.num_outlier_centroids, num_res_centroids=self.num_res_centroids,
             padding=self.padding, outlier_padding=self.outlier_padding, num_codebooks=self.num_codebooks,
             group_size=self.group_size, outlier_size=self.outlier_size, vector_len=self.vector_len,
-            outlier_vector_len=self.outlier_vector_len, vector_quant_dim=self.vector_quant_dim)
+            outlier_vector_len=self.outlier_vector_len, vector_quant_dim=self.vector_quant_dim,
+            _quant_grad=getattr(self, "_quant_grad", False))
 
     def proxy_error_forward(self, W, H):
         """diff^T diff * H with diff = dequant() - W (the quantizer's layer-wise proxy loss)."""
@@ -265,7 +324,8 @@ class VQuantLinear(nn.Module):
         return diff.T @ diff * H
 
     def set_centroids_grad(self, requires_grad: bool) -> None:
-        """Sets `requires_grad` on the codebooks (reference surface); the CUDA path computes no codebook gradient."""
+        """Sets `requires_grad` on the codebooks (reference surface).  They receive gradients once the module has
+        opted in with `set_quant_grad(True)`; without it the CUDA path computes no codebook gradient."""
         self.centroids.weight.requires_grad = requires_grad
         if self.enable_outlier:
             self.outlier_centroids.weight.requires_grad = requires_grad

@@ -33,6 +33,13 @@ EXPORTS = (
     "vptq_b200_lists_build_host", "vptq_b200_quant_gemv_multi_ws", "vptq_b200_tp_untag", "vptq_b200_lists_deal_host",
 )
 
+# training entry points (include/vptq_b200_grad.h), exported from the same library
+GRAD_EXPORTS = ("vptq_b200_grad_version", "vptq_b200_grad_workspace_bytes", "vptq_b200_quant_gemm_wgrad",
+                "vptq_b200_dequant_backward")
+GRAD_VERSION = 1
+GRAD_OP_WGRAD, GRAD_OP_DEQUANT_BACKWARD, GRAD_OP_WGRAD_GENERIC = 0, 1, 2
+GRAD_FLAG_GENERIC = 1
+
 MAX_FUSED, MAX_RANKS = 4, 8
 
 
@@ -67,6 +74,17 @@ class LinearDesc(ctypes.Structure):
         ("lists_tile_cols", ctypes.c_int32), ("lists_reserved", ctypes.c_int32),
     ]
 
+
+class LinearGrads(ctypes.Structure):
+    """struct vptq_linear_grads (include/vptq_b200_grad.h): one output pointer per gradient, NULL = not wanted."""
+    _fields_ = [
+        ("struct_size", ctypes.c_uint32), ("reserved", ctypes.c_uint32),
+        ("centroids", ctypes.c_void_p), ("res_centroids", ctypes.c_void_p), ("outlier_centroids", ctypes.c_void_p),
+        ("weight_scale", ctypes.c_void_p), ("weight_bias", ctypes.c_void_p),
+    ]
+
+
+GRAD_FIELDS = ("centroids", "res_centroids", "outlier_centroids", "weight_scale", "weight_bias")
 
 _lib = None
 _lock = threading.Lock()
@@ -120,6 +138,19 @@ def lib() -> ctypes.CDLL:
             getattr(L, f).restype = ctypes.c_int
         if L.vptq_b200_abi_version() != ABI_VERSION:
             raise RuntimeError(f"libvptq_b200.so ABI {L.vptq_b200_abi_version()} != expected {ABI_VERSION}")
+        for f in GRAD_EXPORTS:
+            if not hasattr(L, f):
+                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_grad.h): rebuild it")
+        gp = ctypes.POINTER(LinearGrads)
+        L.vptq_b200_grad_version.restype = ctypes.c_int
+        L.vptq_b200_grad_workspace_bytes.restype = ctypes.c_size_t
+        L.vptq_b200_grad_workspace_bytes.argtypes = [dp, i32, i32]
+        L.vptq_b200_quant_gemm_wgrad.argtypes = [dp, vp, i64, vp, i64, i32, gp, vp, sz, u32, vp]
+        L.vptq_b200_quant_gemm_wgrad.restype = ctypes.c_int
+        L.vptq_b200_dequant_backward.argtypes = [dp, vp, i64, gp, vp, sz, u32, vp]
+        L.vptq_b200_dequant_backward.restype = ctypes.c_int
+        if L.vptq_b200_grad_version() != GRAD_VERSION:
+            raise RuntimeError(f"libvptq_b200.so grad interface {L.vptq_b200_grad_version()} != expected {GRAD_VERSION}")
         _lib = L
     return _lib
 
@@ -247,6 +278,12 @@ def workspace(device: torch.device, nbytes: int) -> torch.Tensor:
     return ws
 
 
+def release_workspaces() -> None:
+    """Drop the cached per-stream workspaces (they only grow: a weight-gradient call can leave hundreds of MB).  The
+    next call allocates a fresh zeroed one.  Not while a captured CUDA graph still uses the old ones."""
+    _workspaces.clear()
+
+
 def workspace_bytes(desc: LinearDesc, tokens: int, op: int) -> int:
     return int(lib().vptq_b200_workspace_bytes(ctypes.byref(desc), int(tokens), int(op)))
 
@@ -277,7 +314,9 @@ def _ws_bytes_cached(desc: LinearDesc, tokens: int, op: int) -> int:
     key = (min(tokens, 4) if op == OP_GEMV else tokens, op)     # the GEMV plans passes of at most 4 tokens
     v = cache.get(key)
     if v is None:
-        v = cache[key] = workspace_bytes(desc, tokens, op)
+        # ("grad", op): an op of vptq_b200_grad_workspace_bytes
+        v = cache[key] = grad_workspace_bytes(desc, tokens, op[1]) if isinstance(op, tuple) else \
+            workspace_bytes(desc, tokens, op)
     return v
 
 
@@ -383,6 +422,63 @@ def quant_gemm_dgrad(desc: LinearDesc, dy2d: torch.Tensor, dx2d: torch.Tensor) -
         rc = lib().vptq_b200_quant_gemm(ctypes.byref(desc), dy2d.data_ptr(), row_pitch(dy2d), dx2d.data_ptr(),
                                         row_pitch(dx2d), tokens, ws.data_ptr(), ws.numel(), FLAG_TRANSPOSE, _stream(dev))
     check(rc, "vptq_b200_quant_gemm (transpose)")
+
+
+def grad_workspace_bytes(desc: LinearDesc, tokens: int, op: int) -> int:
+    return int(lib().vptq_b200_grad_workspace_bytes(ctypes.byref(desc), int(tokens), int(op)))
+
+
+def make_grads(grads: dict) -> LinearGrads:
+    """{field of GRAD_FIELDS: output tensor} -> struct vptq_linear_grads (missing fields = not wanted)."""
+    unknown = set(grads) - set(GRAD_FIELDS)
+    if unknown:
+        raise RuntimeError(f"unknown gradient outputs {sorted(unknown)}; expected some of {GRAD_FIELDS}")
+    g = LinearGrads()
+    g.struct_size = ctypes.sizeof(LinearGrads)
+    for k, t in grads.items():
+        if t is not None:
+            require_cuda(k, t)
+            setattr(g, k, t.data_ptr())
+    return g
+
+
+def _dense_rows(t: torch.Tensor) -> torch.Tensor:
+    # autograd hands over expanded (zero-stride) gradients, e.g. from y.sum(): the kernels need pitch >= columns
+    if t.stride(-1) != 1 or (t.shape[0] > 1 and t.stride(0) < t.shape[1]):
+        return t.contiguous()
+    return t
+
+
+def quant_gemm_wgrad(desc: LinearDesc, x2d: torch.Tensor, dy2d: torch.Tensor, grads: dict, flags: int = 0) -> None:
+    """Weight gradients of y = x W^T + bias into the tensors of `grads` (vptq_b200_quant_gemm_wgrad):
+    x2d [tokens, in_features], dy2d [tokens, out_features].  flags=GRAD_FLAG_GENERIC takes the generic route (G in
+    the workspace + scatter kernel) also where the fused GEMM epilogue applies; the results are bit-identical."""
+    x2d, dy2d = _dense_rows(x2d), _dense_rows(dy2d)
+    tokens = x2d.shape[0]
+    if dy2d.shape[0] != tokens:
+        raise RuntimeError(f"x has {tokens} rows but dy has {dy2d.shape[0]}")
+    g = make_grads(grads)
+    dev = dy2d.device
+    with _on_device(dev):
+        op = GRAD_OP_WGRAD_GENERIC if flags & GRAD_FLAG_GENERIC else GRAD_OP_WGRAD
+        ws = workspace(dev, _ws_bytes_cached(desc, tokens, ("grad", op)))
+        rc = lib().vptq_b200_quant_gemm_wgrad(ctypes.byref(desc), x2d.data_ptr(), row_pitch(x2d), dy2d.data_ptr(),
+                                              row_pitch(dy2d), tokens, ctypes.byref(g), ws.data_ptr(), ws.numel(),
+                                              int(flags), _stream(dev))
+    check(rc, "vptq_b200_quant_gemm_wgrad")
+
+
+def dequant_backward(desc: LinearDesc, dw: torch.Tensor, grads: dict) -> None:
+    """Gradients of the layer's tensors from the gradient dw [out_features, in_features] of dequant()'s output
+    (vptq_b200_dequant_backward)."""
+    dw = _dense_rows(dw)
+    g = make_grads(grads)
+    dev = dw.device
+    with _on_device(dev):
+        ws = workspace(dev, _ws_bytes_cached(desc, 1, ("grad", GRAD_OP_DEQUANT_BACKWARD)))
+        rc = lib().vptq_b200_dequant_backward(ctypes.byref(desc), dw.data_ptr(), row_pitch(dw), ctypes.byref(g),
+                                              ws.data_ptr(), ws.numel(), 0, _stream(dev))
+    check(rc, "vptq_b200_dequant_backward")
 
 
 def dequant(desc: LinearDesc, w_out: torch.Tensor) -> None:

@@ -65,8 +65,12 @@ def dequant(
     vector_len: int,
     outlier_vector_len: int,
     vector_quant_dim: str = "out",
+    _quant_grad: bool = False,
 ) -> torch.Tensor:
-    """Dense weight [out_features, in_features] (reference: vptq/ops/quant_gemm.py:43-158)."""
+    """Dense weight [out_features, in_features] (reference: vptq/ops/quant_gemm.py:43-158).
+
+    `_quant_grad` (VQuantLinear.set_quant_grad): under grad mode the result is differentiable with respect to the
+    codebooks, weight_scale and weight_bias that require grad (vptq_b200_dequant_backward)."""
     if vector_quant_dim == "in":
         raise ValueError("Not implemented yet.")
     if not is_indice_packed:
@@ -86,9 +90,58 @@ def dequant(
         num_centroids=num_centroids, num_outlier_centroids=num_outlier_centroids,
         num_res_centroids=num_res_centroids, group_size=group_size, outlier_size=outlier_size,
         in_features=in_features, out_features=out_features, derive=False, lists=False)
+    if _quant_grad and torch.is_grad_enabled():
+        slots = _quant_slots(centroids, res_centroids if enable_residual else None,
+                             outlier_centroids if enable_outlier else None, weight_scale if enable_norm else None,
+                             weight_bias if enable_norm else None)
+        if any(t.requires_grad for _, t in slots):
+            others = [t for t in (indices, outlier_indices if enable_outlier else None,
+                                  perm if enable_perm else None) if t is not None]
+            return _DequantFn.apply([desc, perm_], out_features, tuple(n for n, _ in slots),
+                                    *[t for _, t in slots], *others)
     w = torch.empty(out_features, in_features, dtype=centroids.dtype, device=centroids.device)
     native.dequant(desc, w)
     return w
+
+
+def _quant_slots(centroids, residual_centroids, outlier_centroids, weight_scale, weight_bias):
+    """(gradient name of vptq_linear_grads, tensor) for the layer's floating-point tensors that are present."""
+    pairs = (("centroids", centroids), ("res_centroids", residual_centroids), ("outlier_centroids", outlier_centroids),
+             ("weight_scale", weight_scale), ("weight_bias", weight_bias))
+    return [(n, t) for n, t in pairs if t is not None]
+
+
+def _quant_grads(ctx, first: int, names, tensors) -> dict:
+    """Output tensors for the quantizer gradients autograd asks for; input slot `first + i` holds tensors[i]."""
+    return {n: torch.empty_like(t, memory_format=torch.contiguous_format)
+            for i, (n, t) in enumerate(zip(names, tensors)) if ctx.needs_input_grad[first + i]}
+
+
+class _DequantFn(torch.autograd.Function):
+    """W = dequant(layer), differentiable with respect to the codebooks, weight_scale and weight_bias.
+
+    backward: vptq_b200_dequant_backward reduces dL/dW into each requested tensor (64-bit fixed point: bit-identical
+    from run to run).  The packed indices, outlier indices and perm are saved too, only for autograd's version
+    check; they get no gradient."""
+
+    @staticmethod
+    def forward(ctx, keep, out_features, names, *layer):
+        ctx.keep, ctx.names = keep, names
+        ctx.save_for_backward(*layer)
+        desc = keep[0]
+        w = torch.empty(out_features, desc.in_features, dtype=layer[0].dtype, device=layer[0].device)
+        native.dequant(desc, w)
+        return w
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dw):
+        saved = ctx.saved_tensors
+        quant = saved[:len(ctx.names)]
+        want = _quant_grads(ctx, 3, ctx.names, quant)
+        if want:
+            native.dequant_backward(ctx.keep[0], dw, want)
+        return (None, None, None) + tuple(want.get(n) for n in ctx.names) + (None,) * (len(saved) - len(quant))
 
 
 def quant_gemm(
@@ -119,8 +172,12 @@ def quant_gemm(
     vector_quant_dim: str = "out",
     _desc_cache: Optional[list] = None,
     _drop_packed: bool = False,
+    _quant_grad: bool = False,
 ) -> torch.Tensor:
-    """y = x @ W^T + bias for one VPTQ layer (reference: vptq/ops/quant_gemm.py:161-275)."""
+    """y = x @ W^T + bias for one VPTQ layer (reference: vptq/ops/quant_gemm.py:161-275).
+
+    `_quant_grad` (VQuantLinear.set_quant_grad): under grad mode the codebooks, weight_scale and weight_bias that
+    require grad get gradients too, also when x does not require grad (vptq_b200_quant_gemm_wgrad)."""
     if vector_quant_dim == "in":
         raise ValueError("Not implemented yet.")
     if not is_indice_packed:
@@ -150,13 +207,23 @@ def quant_gemm(
     x2d = x.reshape(-1, in_features)
     if x2d.stride(-1) != 1 or (x2d.shape[0] > 1 and x2d.stride(0) < in_features):
         x2d = x2d.contiguous()    # broadcast rows (expand, overlapping unfold windows): the kernels need pitch >= I
-    if torch.is_grad_enabled() and x.requires_grad:
-        # keeps the descriptor (and the uint16 perm it points to) alive until backward, also for a one-off descriptor
-        keep = _desc_cache[:2] if _desc_cache is not None else [desc, perm_]
-        layer = (indices, centroids, residual_centroids, outlier_indices, outlier_centroids, perm, weight_scale,
-                 weight_bias)
-        y = _QuantLinearFn.apply(x2d, bias, keep, out_features, *[t for t in layer if t is not None])
-        return y.reshape(*x.shape[:-1], out_features)
+    if torch.is_grad_enabled():
+        slots = _quant_slots(centroids, residual_centroids, outlier_centroids, weight_scale, weight_bias) \
+            if _quant_grad else []
+        quant = any(t.requires_grad for _, t in slots)
+        if x.requires_grad or quant:
+            # keeps the descriptor (and the uint16 perm it points to) alive until backward, also for a one-off
+            # descriptor
+            keep = _desc_cache[:2] if _desc_cache is not None else [desc, perm_]
+            if not quant:
+                layer = (indices, centroids, residual_centroids, outlier_indices, outlier_centroids, perm,
+                         weight_scale, weight_bias)
+                y = _QuantLinearFn.apply(x2d, bias, keep, out_features, *[t for t in layer if t is not None])
+            else:
+                others = [t for t in (indices, outlier_indices, perm) if t is not None]
+                y = _QuantLinearWgradFn.apply(x2d, bias, keep, out_features, tuple(n for n, _ in slots),
+                                              *[t for _, t in slots], *others)
+            return y.reshape(*x.shape[:-1], out_features)
     return _forward(desc, x2d, out_features).reshape(*x.shape[:-1], out_features)
 
 
@@ -191,18 +258,56 @@ class _QuantLinearFn(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, dy):
         ctx.saved_tensors            # version check of the layer tensors
-        desc = ctx.keep[0]
-        if not desc.indices:
-            raise RuntimeError("backward through a decode-only VQuantLinear (prepare(drop_packed=True)): the input "
-                               "gradient needs the packed index words, which were freed; reload the checkpoint")
-        dx = dbias = None
-        if ctx.needs_input_grad[0]:
-            dx = torch.empty(dy.shape[0], desc.in_features, dtype=dy.dtype, device=dy.device)
-            if dy.shape[0]:
-                native.quant_gemm_dgrad(desc, dy, dx)
-        if ctx.needs_input_grad[1]:
-            dbias = dy.float().sum(0).to(dy.dtype)
+        dx, dbias = _input_grads(ctx, ctx.keep[0], dy)
         return (dx, dbias, None, None) + (None,) * len(ctx.saved_tensors)
+
+
+def _input_grads(ctx, desc, dy):
+    """(dX, dbias) of y = x W^T + bias for the slots 0 and 1 that need them."""
+    if not desc.indices:
+        raise RuntimeError("backward through a decode-only VQuantLinear (prepare(drop_packed=True)): the input "
+                           "gradient needs the packed index words, which were freed; reload the checkpoint")
+    dx = dbias = None
+    if ctx.needs_input_grad[0]:
+        dx = torch.empty(dy.shape[0], desc.in_features, dtype=dy.dtype, device=dy.device)
+        if dy.shape[0]:
+            native.quant_gemm_dgrad(desc, dy, dx)
+    if ctx.needs_input_grad[1]:
+        dbias = dy.float().sum(0).to(dy.dtype)
+    return dx, dbias
+
+
+class _QuantLinearWgradFn(torch.autograd.Function):
+    """_QuantLinearFn plus the gradients of the codebooks, weight_scale and weight_bias (VQuantLinear.set_quant_grad).
+
+    forward: the same no-grad routing (bit-identical values); x is saved for the weight gradient.
+    backward: dX and dbias as _QuantLinearFn; the quantizer tensors autograd asks for through
+    vptq_b200_quant_gemm_wgrad (G = dY^T x by the wgmma GEMM, reduced in 64-bit fixed point: bit-identical from run
+    to run).  `layer` = the quantizer tensors named by `names`, then the index tensors and perm (saved only for
+    autograd's version check)."""
+
+    @staticmethod
+    def forward(ctx, x2d, bias, keep, out_features, names, *layer):
+        ctx.keep, ctx.names = keep, names
+        ctx.save_for_backward(x2d, *layer)
+        return _forward(keep[0], x2d, out_features)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        saved = ctx.saved_tensors
+        x2d, quant = saved[0], saved[1:1 + len(ctx.names)]
+        desc = ctx.keep[0]
+        dx, dbias = _input_grads(ctx, desc, dy)
+        want = _quant_grads(ctx, 5, ctx.names, quant)
+        if want:
+            if dy.shape[0]:
+                native.quant_gemm_wgrad(desc, x2d, dy, want)
+            else:
+                for t in want.values():
+                    t.zero_()
+        return (dx, dbias, None, None, None) + tuple(want.get(n) for n in ctx.names) + \
+            (None,) * (len(saved) - 1 - len(quant))
 
 
 def quant_gemv_v2(
