@@ -125,8 +125,15 @@ typedef struct vptq_linear_desc {
 
   /* Optional second load-time derivative: the SAME indices re-bucketed into slice x tile lists for the
      decode kernel that keeps 64 KiB slices of a large main codebook in each SM's shared memory
-     (NULL = not provided: the packed words above are decoded directly; results agree up to fp32
-     summation order and one fp16 rounding of c + r, which is what the reference's kernel does too).
+     (NULL = not provided: the packed words above are decoded directly).  With the lists, single-token
+     results round x * weight_scale to the layer's 16-bit type and, for fp16 layers, c + r to fp16, as
+     the reference's kernel does, and sum in fp32 per unit, then in 2^-30 fixed point over the Q = NS * NT
+     units of an output: an absolute error of up to Q * 2^-31 per output whatever its size.  By default
+     the fixed point holds |output| < 2^33 only and carries no inf or NaN: with non-finite inputs or layer
+     tensors, or unit sums past that range, these results are not defined.  With the environment variable
+     VPTQ_B200_LISTS_CHECKED=1 (read at each launch) the kernel keeps such sums out of the fixed point and
+     returns +inf, -inf or NaN for them (NaN for finite sums past 2^33 / 2^ceil(log2 Q)), like the other
+     routes, at a cost of about 2 % of decode throughput.
      Eligible layers: vector_len 8, one codebook group, no outlier columns, K = NS * 4096 with
      2 <= NS <= 16, Kr <= 256; used for single-token calls.  Geometry:
        NT  = ceil(I / 4096) column tiles over the ORIGINAL input features,

@@ -107,8 +107,8 @@ def probe_expect(L, route, block_rows=2048):
         else:
             if dt == "fp16":   # x' = x * s in fp16 (exact), c + r in packed fp16
                 xq, c = s, _fp16(main.astype(np.float64) + res)
-            else:              # x' = x * s rounded to fp16, c + r in fp32
-                xq, c = _fp16(s), _f32(main + res)
+            else:              # x' = x * s in bf16 (exact), c + r in fp32
+                xq, c = s, _f32(main + res)
             p = _f32(c.astype(np.float64) * xq)
             q = _lists_fixed(p, wb, sl, has_norm)
             y = _f32(q) * np.float32(1.0 / _FIX)

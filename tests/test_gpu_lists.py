@@ -2,9 +2,11 @@
 
 Each case is run twice on the same tensors -- descriptor with the slice x tile lists (shared-memory
 gathers) and without (generic kernel, L1/L2 gathers) -- and both are held to the oracle bar
-(max|y - y*| / max|y*| <= 1e-3 fp16, 4e-3 bf16).  The list kernel rounds c + r and x * scale to fp16 exactly
-as the reference's kernel does (csrc/kernels/quant_gemv.cuh:56,124-127) and accumulates in fp32; the generic
-kernel keeps those in fp32, so the two agree to a few output ulps, far inside the bar."""
+(max|y - y*| / max|y*| <= 1e-3 fp16, 4e-3 bf16).  The list kernel rounds x * scale to the layer's 16-bit type and,
+for fp16 layers, c + r to fp16, exactly as the reference's kernel does (csrc/kernels/quant_gemv.cuh:56,124-127), and
+accumulates in fp32, then in 2^-30 fixed point across units (an absolute floor of Q * 2^-31 per output); the
+generic kernel keeps those in fp32, so the two agree to a few output ulps, far inside the bar.  Non-finite and
+out-of-range values: tests/test_gpu_extremes.py."""
 import numpy as np
 import pytest
 import torch

@@ -455,7 +455,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
 #pragma unroll
     for (int e = 0; e < V; ++e) acc[t][e] = 0.f;
 
-  // field j of ring stage `sw` (0 for lanes past the end: they gather entry 0 and multiply by zero)
+  // field j of ring stage `sw` (0 for lanes past the end: they gather entry 0 and skip the FMAs)
   auto field_at = [&](const uint32_t* sw, int j, int nf) -> uint32_t {
     const uint32_t bit = uint32_t(j) * uint32_t(b);
     const uint32_t w = bit >> 5;
@@ -571,7 +571,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
     // row boundaries always fall between U-blocks (rows are padded to whole blocks).
     const int gps = pl.seg_fields >> 5;                 // groups per ring segment (multiple of U)
     const int ngu = ((wcols + 32 * U - 1) / (32 * U)) * U;  // groups per unit, padded to whole U-blocks
-    const int NG = nunits * ngu;                        // (padding groups decode to field 0, x' = 0)
+    const int NG = nunits * ngu;                        // (padding groups decode to field 0, no FMA)
     uint32_t fld[U];
     uint32_t cw[U][V / 2];
     // load side: position of the next group to fetch
@@ -607,10 +607,11 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
         const int j = (c_gl + k) * 32 + lane;  // this lane's field, relative to the warp's sub-range
         uint32_t rw[V / 2];
         if constexpr (RES) lds_entry<V>(rw, s_res_lane + (fld[k] >> p.ib) * res_stride);
+        // lanes past the end gathered entry 0 of both codebooks: they add nothing (not even 0 * entry, which an
+        // inf or NaN there would turn into NaN in rows that never use the entry)
+        if (j < wcols) {
 #pragma unroll
-        for (int t = 0; t < NT; ++t) {
-          const float xv = j < wcols ? sx[t * pl.sx_stride + sf0 + j] : 0.f;
-          fma_entry<T, V, RES>(acc[t], xv, cw[k], rw);
+          for (int t = 0; t < NT; ++t) fma_entry<T, V, RES>(acc[t], sx[t * pl.sx_stride + sf0 + j], cw[k], rw);
         }
         if (n0 + k + U < NG) load(fld[k], cw[k]);  // refill the slot: group n0+k+U
       }

@@ -24,7 +24,9 @@
 //   * a unit that lies inside one warp's run is reduced with 9 shuffles; the (at most two) units a run shares
 //     with its neighbours are parked in shared memory and merged in warp order;
 //   * reduction over the Q = NS * NT combos of a row: every unit adds its 8 sums, converted to 2^-30 fixed
-//     point, into a 64-bit accumulator row in the workspace with red.global.add.u64.  Integer addition is
+//     point, into a 64-bit accumulator row in the workspace with red.global.add.u64 (sums that are not finite or
+//     out of the range that keeps Q of them from wrapping leave their class in a per-row record instead, which
+//     the conversion turns into +-inf / NaN, see add_unit).  Integer addition is
 //     associative, so the result does not depend on the arrival order: bit-identical from run to run, like
 //     an ordered sum, without a partial-sum table (a last-arriver that adds Q partials per output was
 //     measured at 4-8 us of tail per launch).  Row blocks of 32 index rows carry an arrival counter (units,
@@ -70,6 +72,10 @@ constexpr int kMaxWindow = 3072;  // units of one CTA (bounds the tab window in 
 constexpr int kRB = 32;           // index rows per arrival counter
 constexpr int kResRep = 8;        // bank-group replication of the residual table
 constexpr uint32_t kStepMask = (1u << 26) - 1u;
+// counter region of the workspace (zero at rest): the arrival counters of every fused layer's row blocks in
+// [0, kClassOffset), the 16-bit class records of their index rows behind them (<= kMaxIndexRows + 4 of them)
+constexpr size_t kClassOffset = 16384;
+static_assert(kClassOffset + (size_t(kMaxIndexRows) + 2 * kMaxFusedLayers) * 2 <= kCounterRegionBytes, "");
 
 struct ListsLayer {
   const uint32_t* stream;  // [T][32] entry words
@@ -82,6 +88,8 @@ struct ListsLayer {
   void* y;
   unsigned long long* yacc;  // [Ro][8] fixed-point (2^-30) accumulators, zero at rest
   uint32_t* counters;        // [ceil(Ro / kRB)], zero at rest
+  uint16_t* cls;             // [Ro] class records of unit sums kept out of yacc (add_unit), zero at rest
+  float lim;                 // unit sums with |v| >= lim (or not finite) are not added as integers
   int I, O, Ro, Kr, NS, Q, TCW, U;
   int ncta;  // CTAs working on this layer
 };
@@ -124,15 +132,33 @@ __device__ __forceinline__ uint32_t mad_u32(uint32_t a, uint32_t b, uint32_t c) 
   asm("mad.lo.u32 %0, %1, %2, %3;" : "=r"(r) : "r"(a), "r"(b), "r"(c));
   return r;
 }
-// fp32 -> 2^-30 fixed point (saturating) and back; |v| < 2^33 is far beyond any 16-bit activation
+// fp32 -> 2^-30 fixed point and back.  The rounding to 2^-30 costs up to 2^-31 per unit, an absolute floor of
+// Q * 2^-31 per output whatever its size (fp16 outputs do not notice it: their smallest step is 2^-24).  Unchecked
+// (the default variant), an inf saturates, a NaN becomes some integer and unit sums that together pass 2^33 wrap the
+// 64-bit sum -- three fp16 products of 60000 x 60000 do, and in bf16 2^33 is an ordinary value.  The checked variant
+// (CHK) admits only |v| < lim = 2^33 / 2^ceil(log2 Q): no sum of Q admitted terms reaches 2^63, so it never wraps;
+// anything else leaves its class in the row's record and the output becomes +inf, -inf or NaN.
 constexpr float kFixScale = 1073741824.f, kFixInv = 1.f / 1073741824.f;
-__device__ __forceinline__ void red_add_fixed(unsigned long long* p, float v) {
-  const long long q = __float2ll_rn(v * kFixScale);
-  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(p), "l"(q) : "memory");
+constexpr uint32_t kClsPosInf = 1u, kClsNegInf = 2u, kClsNaN = 3u;  // OR of two classes = class of their sum
+// Unit sum v of output e of index row `row` joins the output: as an integer when it is in range, otherwise as its
+// class (+inf, -inf, NaN or out of range) in the row's 16-bit record (2 bits per output), read at the conversion.
+__device__ __forceinline__ void record_class(uint16_t* rec, int e, float v) {
+  const uint32_t c = v == INFINITY ? kClsPosInf : v == -INFINITY ? kClsNegInf : kClsNaN;
+  const uintptr_t a = reinterpret_cast<uintptr_t>(rec);  // 16-bit record inside a 32-bit word
+  atomicOr(reinterpret_cast<unsigned int*>(a & ~uintptr_t(3)), c << (uint32_t(a & 2u) * 8u + 2u * uint32_t(e)));
+}
+// CHK = false (the default kernel): no range check, as before -- non-finite or out-of-range sums give undefined
+// (finite or wrongly signed) outputs; CHK = true: VPTQ_B200_LISTS_CHECKED=1, see gemv_lists_launch.
+template <bool CHK>
+__device__ __forceinline__ void add_unit(const ListsLayer& L, int row, int e, float v) {
+  const bool in_range = !CHK || fabsf(v) < L.lim;  // (false for inf and NaN)
+  const long long q = __float2ll_rn((in_range ? v : 0.f) * kFixScale);
+  asm volatile("red.global.add.u64 [%0], %1;" ::"l"(L.yacc + size_t(row) * 8 + e), "l"(q) : "memory");
+  if (!in_range) record_class(L.cls + row, e, v);
 }
 // acc[e] += x' * (c[e] + r[e]).  fp16: c + r in packed fp16 (the reference's ADD2), fp32 accumulation: the
 // fp16 x fp16 product is exact in fp32, so widening both factors and one fp32 FMA round exactly once.
-// bf16: c + r and the product in fp32 (x' is kept as fp16 in shared memory for both dtypes).
+// bf16: x' is bf16 (the reference's input_v), c + r and the product in fp32.
 template <typename T, bool RES>
 __device__ __forceinline__ void fma_entry(float (&acc)[8], uint16_t xh, const uint32_t (&cw)[4], const uint32_t (&rw)[4]) {
   if constexpr (std::is_same<T, __half>::value) {
@@ -144,7 +170,7 @@ __device__ __forceinline__ void fma_entry(float (&acc)[8], uint16_t xh, const ui
       acc[2 * i + 1] = fmaf(xv, c.y, acc[2 * i + 1]);
     }
   } else {
-    const float xv = __half2float(__ushort_as_half(xh));
+    const float xv = __uint_as_float(uint32_t(xh) << 16);
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       float2 c = DT<T>::unpack2(cw[i]);
@@ -191,7 +217,7 @@ __device__ __forceinline__ uint4 load8_tagged(const void* xl, int f, uint32_t ta
   return make_uint4(a.x, a.z, b.x, b.z);
 }
 
-// x' = x * scale for 8 features (stored as fp16) and sum x * wbias (fp32)
+// x' = x * scale for 8 features (stored in the layer's 16-bit type) and sum x * wbias (fp32)
 template <typename T>
 __device__ __forceinline__ uint4 make_xq(const uint4& xr, const uint4& sc, const uint4& wb, bool with_bias, float& bs) {
   const uint32_t xs[4] = {xr.x, xr.y, xr.z, xr.w}, ss[4] = {sc.x, sc.y, sc.z, sc.w}, ws[4] = {wb.x, wb.y, wb.z, wb.w};
@@ -199,14 +225,13 @@ __device__ __forceinline__ uint4 make_xq(const uint4& xr, const uint4& sc, const
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const float2 xf = DT<T>::unpack2(xs[i]);
+    // the product rounded to the 16-bit type, as the reference forms input_v (csrc/kernels/quant_gemv.cuh:56)
     if constexpr (std::is_same<T, __half>::value) {
-      // the product rounded to fp16, as the reference forms input_v (csrc/kernels/quant_gemv.cuh:56)
       __half2 p = __hmul2(*reinterpret_cast<const __half2*>(&xs[i]), *reinterpret_cast<const __half2*>(&ss[i]));
       o[i] = *reinterpret_cast<uint32_t*>(&p);
-    } else {
+    } else {  // (the fp32 product of two bf16 values is exact: one rounding)
       const float2 sf = DT<T>::unpack2(ss[i]);
-      __half2 p = __floats2half2_rn(xf.x * sf.x, xf.y * sf.y);
-      o[i] = *reinterpret_cast<uint32_t*>(&p);
+      o[i] = DT<T>::pack2(xf.x * sf.x, xf.y * sf.y);
     }
     if (with_bias) {
       const float2 wf = DT<T>::unpack2(ws[i]);
@@ -217,7 +242,7 @@ __device__ __forceinline__ uint4 make_xq(const uint4& xr, const uint4& sc, const
   return make_uint4(o[0], o[1], o[2], o[3]);
 }
 
-template <typename T, bool RES>
+template <typename T, bool RES, bool CHK>
 __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constant__ ListsParams mp) {
   extern __shared__ __align__(128) uint8_t smem[];
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -283,6 +308,7 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
         tma_bulk_g2s(s_slice + kSliceBytes + off, cb + size_t(sB) * kSliceBytes + off, 32768u, &bars[1], pol_keep);
     }
     *s_ndone = 0;
+    *reinterpret_cast<uint4*>(smem + mp.off_red + 144) = make_uint4(0u, 0u, 0u, 0u);  // zero entry (padding lanes)
   } else if (tid >= 2 && tid < 2 + kLW * stages) {
     mbar_init(&bars[tid], 1);
     fence_mbar_init();
@@ -426,6 +452,7 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
   if (nstage > 0) {
     const uint32_t res_lane = smem_u32(s_res) + uint32_t(lane & (kResRep - 1)) * 16u;
     const uint32_t ring_lane = smem_u32(ring) + uint32_t(lane) * 4u;
+    const uint32_t s_zero = smem_u32(smem + mp.off_red + 144);  // 16 zero bytes
     // the unit this run starts in: the last i with first(i) <= t_begin (every unit has >= 1 step)
     int u;
     {
@@ -450,7 +477,7 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
       const float mine = warp_reduce_to_lane<8>(acc, lane);
       const bool boundary = u == uF || !complete || u_end >= t_end;
       if (!boundary) {
-        if (lane < 8) red_add_fixed(L.yacc + size_t(u < nA ? rA0 + u : u - nA) * 8 + lane, mine + cb);
+        if (lane < 8) add_unit<CHK>(L, u < nA ? rA0 + u : u - nA, lane, mine + cb);
       } else {
         const int k = warp * 2 + (u == uF ? 0 : 1);
         if (lane < 8) s_piece[k * 8 + lane] = mine;
@@ -474,8 +501,9 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
     //   KEND = k in 1..kSPS (full batches only): the current unit ends with the batch's k-th step and the next
     //             one does not end inside the batch -- the flush sits at a fixed place, no per-step test
     //   KEND < 0: generic (partial batches at the end of a run / segment, units shorter than a batch)
-    auto batch = [&](auto kend_tag, int cnt, uint32_t st) {
+    auto batch = [&](auto kend_tag, auto mask_tag, int cnt, uint32_t st) {
       constexpr int KEND = decltype(kend_tag)::value;
+      constexpr bool MASK = decltype(mask_tag)::value;  // entry 0 is not harmless: padding lanes read zeros
       constexpr bool FULL = KEND >= 0;
       uint32_t ent[kSPS];
       uint32_t cw[kSPS][4], rw[kSPS][4];
@@ -487,9 +515,13 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
       for (int j = 0; j < kSPS; ++j) {
         if (FULL || j < cnt) {
           // entry = index12 | column12 << 12 | residual8 << 24; x_base is 8 KiB aligned, so `|` adds
-          lds_entry<8>(cw[j], mad_u32(ent[j] & 0xfffu, 16u, slice_base));
-          if constexpr (RES) lds_entry<8>(rw[j], mad_u32(ent[j] >> 24, 128u, res_lane));
-          xh[j] = lds_u16(x_base | ((ent[j] >> 11) & 0x1ffeu));
+          uint32_t a_c = mad_u32(ent[j] & 0xfffu, 16u, slice_base), a_r = mad_u32(ent[j] >> 24, 128u, res_lane),
+                   a_x = x_base | ((ent[j] >> 11) & 0x1ffeu);
+          if (MASK && j == KEND - 1 && uint32_t(lane) >= tail) a_c = a_r = a_x = s_zero;  // padding words: below
+          lds_entry<8>(cw[j], a_c);
+          if constexpr (RES) lds_entry<8>(rw[j], a_r);
+          xh[j] = lds_u16(a_x);
+          if (!MASK && j == KEND - 1 && uint32_t(lane) >= tail) xh[j] = 0;
         }
       }
       if constexpr (KEND == 0) {
@@ -499,9 +531,10 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
       } else if constexpr (KEND > 0) {
 #pragma unroll
         for (int j = 0; j < kSPS; ++j) {
-          uint16_t xv = xh[j];
-          if (j == KEND - 1 && uint32_t(lane) >= tail) xv = 0;  // last step of the unit: mask the padding entries
-          fma_entry<T, RES>(acc, xv, cw[j], rw[j]);
+          // the padding words of a unit's last step decode to slice entry 0 and residual entry 0; their lanes have
+          // x' = 0 (above), which adds exactly nothing where x' * 0 is 0 (pad_safe below), and otherwise (MASK) they
+          // read a zero entry instead: not 0 * entry, which an inf or NaN there would turn into NaN in every row
+          fma_entry<T, RES>(acc, xh[j], cw[j], rw[j]);
           if (j == KEND - 1) {
             flush(true);
             advance();
@@ -513,9 +546,11 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
         for (int j = 0; j < kSPS; ++j) {
           if (j < cnt) {
             const bool last = t + 1 == u_end;
-            uint16_t xv = xh[j];
-            if (last && uint32_t(lane) >= tail) xv = 0;
-            fma_entry<T, RES>(acc, xv, cw[j], rw[j]);
+            if (MASK) {
+              if (!last || uint32_t(lane) < tail) fma_entry<T, RES>(acc, xh[j], cw[j], rw[j]);  // (padding: no FMA)
+            } else {
+              fma_entry<T, RES>(acc, (last && uint32_t(lane) >= tail) ? uint16_t(0) : xh[j], cw[j], rw[j]);
+            }
             ++t;
             if (last) {
               flush(true);
@@ -525,6 +560,22 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
         }
       }
     };
+    // Padding lanes are harmless unless entry 0 of a staged slice, with residual entry 0, gives a non-finite
+    // c + r: then x' = 0 times it is NaN.  Each warp checks that once, by the same arithmetic, and only then runs
+    // the main loop that masks the padding lanes' gathers (MASK), so the usual loop carries no extra work.
+    auto pad_harmless = [&](uint32_t slice) {
+      uint32_t c[4], r[4] = {0u, 0u, 0u, 0u};
+      lds_entry<8>(c, slice);
+      if constexpr (RES) lds_entry<8>(r, smem_u32(s_res));
+      float z[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+      fma_entry<T, RES>(z, uint16_t(0), c, r);
+      bool ok = true;
+#pragma unroll
+      for (int e = 0; e < 8; ++e) ok = ok && z[e] == 0.f;
+      return ok;
+    };
+    const bool pad_safe = !CHK || pad_harmless(smem_u32(s_slice)) && (!two || pad_harmless(smem_u32(s_slice) + kSliceBytes));
+    auto main_loop = [&](auto mask_tag) {
 #pragma unroll 1
     for (int part = 0; part < 2; ++part) {
       // part 0 = this run's steps in segment A, part 1 = its steps in segment B (a stage never straddles both)
@@ -544,16 +595,16 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
           const int cnt = min(kSPS, pe - t);
           const int k = u_end - t;  // steps left in the current unit (>= 1)
           if (cnt == kSPS && k > kSPS) {
-            batch(std::integral_constant<int, 0>{}, cnt, st);
+            batch(std::integral_constant<int, 0>{}, mask_tag, cnt, st);
           } else if (cnt == kSPS && !(u + 1 < nun && int(s_tab[u + 2] & kStepMask) - t <= kSPS)) {
             switch (k) {
-              case 1: batch(std::integral_constant<int, 1>{}, cnt, st); break;
-              case 2: batch(std::integral_constant<int, 2>{}, cnt, st); break;
-              case 3: batch(std::integral_constant<int, kEnd3>{}, cnt, st); break;
-              default: batch(std::integral_constant<int, kSPS>{}, cnt, st); break;
+              case 1: batch(std::integral_constant<int, 1>{}, mask_tag, cnt, st); break;
+              case 2: batch(std::integral_constant<int, 2>{}, mask_tag, cnt, st); break;
+              case 3: batch(std::integral_constant<int, kEnd3>{}, mask_tag, cnt, st); break;
+              default: batch(std::integral_constant<int, kSPS>{}, mask_tag, cnt, st); break;
             }
           } else {
-            batch(std::integral_constant<int, -1>{}, cnt, st);
+            batch(std::integral_constant<int, -1>{}, mask_tag, cnt, st);
           }
         }
         __syncwarp();  // every lane has read its words of the stage: refill it
@@ -561,6 +612,9 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
         if (++slot == stages) slot = 0, par ^= 1u;
       }
     }
+    };
+    if (pad_safe) main_loop(std::false_type{});
+    else main_loop(std::true_type{});
     // the run ended inside a unit: its sums so far are this warp's piece of that unit
     if (u < nun && int(s_tab[u] & kStepMask) < t_end) flush(false);
   }
@@ -595,7 +649,7 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
           if (pj != un) break;
           v += s_piece[j * 8 + e];
         }
-        red_add_fixed(L.yacc + size_t(un < nA ? rA0 + un : un - nA) * 8 + e, v + (un >= nA ? cbiasB : cbiasA));
+        add_unit<CHK>(L, un < nA ? rA0 + un : un - nA, e, v + (un >= nA ? cbiasB : cbiasA));
       }
     }
   }
@@ -632,16 +686,23 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
       if (r < Ro) {
         unsigned long long* p = L.yacc + size_t(r) * 8;
         long long q[8];
+        uint16_t cls = 0;  // (loaded with the accumulators: one round trip to L2, not two)
+        if (CHK) asm volatile("ld.global.cg.u16 %0, [%1];" : "=h"(cls) : "l"(L.cls + r) : "memory");
 #pragma unroll
         for (int k = 0; k < 4; ++k)
           asm volatile("ld.global.cg.v2.u64 {%0, %1}, [%2];" : "=l"(q[2 * k]), "=l"(q[2 * k + 1]) : "l"(p + 2 * k) : "memory");
 #pragma unroll
         for (int k = 0; k < 4; ++k) *reinterpret_cast<ulonglong2*>(p + 2 * k) = make_ulonglong2(0ull, 0ull);  // zero at rest
+        // (rows 2i and 2i + 1 share a 32-bit record word; both are converted here, after every unit has arrived)
+        if (CHK && cls) L.cls[r] = 0;
         const int o = r * 8;
         float v[8];
 #pragma unroll
-        for (int e = 0; e < 8; ++e)
-          v[e] = float(q[e]) * kFixInv + ((bias && o + e < L.O) ? DT<T>::to_float(bias[o + e]) : 0.f);
+        for (int e = 0; e < 8; ++e) {
+          const uint32_t c = (uint32_t(cls) >> (2 * e)) & 3u;
+          const float s = c == 0u ? float(q[e]) * kFixInv : c == kClsPosInf ? INFINITY : c == kClsNegInf ? -INFINITY : NAN;
+          v[e] = s + ((bias && o + e < L.O) ? DT<T>::to_float(bias[o + e]) : 0.f);
+        }
         if (o + 8 <= L.O && (reinterpret_cast<uintptr_t>(y) & 15u) == 0) {
           const uint4 pk = make_uint4(DT<T>::pack2(v[0], v[1]), DT<T>::pack2(v[2], v[3]), DT<T>::pack2(v[4], v[5]),
                                       DT<T>::pack2(v[6], v[7]));
@@ -713,12 +774,13 @@ __global__ void tp_untag_kernel(const void* tagged, uint4* y, int n8, const uint
 using ListsKernelFn = void (*)(const ListsParams);
 
 template <typename T>
-ListsKernelFn pick_lists_t(bool res) {
-  return res ? gemv_lists_kernel<T, true> : gemv_lists_kernel<T, false>;
+ListsKernelFn pick_lists_t(bool res, bool chk) {
+  if (chk) return res ? gemv_lists_kernel<T, true, true> : gemv_lists_kernel<T, false, true>;
+  return res ? gemv_lists_kernel<T, true, false> : gemv_lists_kernel<T, false, false>;
 }
-ListsKernelFn pick_lists(int dtype, bool res) {
-  if (dtype == VPTQ_FP16) return pick_lists_t<__half>(res);
-  if (dtype == VPTQ_BF16) return pick_lists_t<__nv_bfloat16>(res);
+ListsKernelFn pick_lists(int dtype, bool res, bool chk) {
+  if (dtype == VPTQ_FP16) return pick_lists_t<__half>(res, chk);
+  if (dtype == VPTQ_BF16) return pick_lists_t<__nv_bfloat16>(res, chk);
   return nullptr;
 }
 
@@ -781,7 +843,12 @@ int gemv_lists_launch(int n, const vptq_linear_desc* const* descs, const void* x
     set_error("gemv_lists: x must be 16-byte aligned");
     return VPTQ_ERR_UNSUPPORTED;
   }
-  ListsKernelFn fn = pick_lists(d0.dtype, res);
+  // VPTQ_B200_LISTS_CHECKED=1: the kernel variant that keeps non-finite and out-of-range unit sums out of the fixed
+  // point (per-output class record) and masks padding lanes whose entry 0 is not harmless.  Off by default: it
+  // costs 1-3 % of decode throughput (DESIGN.md section 3).  Read at every launch (a graph captures the variant).
+  const char* chk_env = std::getenv("VPTQ_B200_LISTS_CHECKED");
+  const bool chk = chk_env && chk_env[0] && std::strcmp(chk_env, "0") != 0;
+  ListsKernelFn fn = pick_lists(d0.dtype, res, chk);
   if (!fn) return VPTQ_ERR_UNSUPPORTED;
   if (int rc = ensure_smem_attr(reinterpret_cast<const void*>(fn), dev->smem_optin)) return rc;
 
@@ -849,7 +916,7 @@ int gemv_lists_launch(int n, const vptq_linear_desc* const* descs, const void* x
     set_error("gemv_lists: %zu index rows exceed %d", rows_total, kMaxIndexRows);
     return VPTQ_ERR_UNSUPPORTED;
   }
-  if (!workspace || workspace_bytes < ws_need || nblk * 4 > kCounterRegionBytes) {
+  if (!workspace || workspace_bytes < ws_need || nblk * 4 > kClassOffset) {
     set_error("gemv_lists: workspace %zu bytes < required %zu", workspace_bytes, ws_need);
     return VPTQ_ERR_WORKSPACE;
   }
@@ -897,7 +964,9 @@ int gemv_lists_launch(int n, const vptq_linear_desc* const* descs, const void* x
   }
   uint32_t begin = 0;
   uint8_t* wsb = reinterpret_cast<uint8_t*>(workspace);
-  size_t part_off = kCounterRegionBytes, ctr_off = 0;
+  size_t part_off = kCounterRegionBytes, ctr_off = 0, cls_off = kClassOffset;
+  int lg_q = 0;
+  while ((1 << lg_q) < Q) ++lg_q;
   for (int l = 0; l < n; ++l) {
     const vptq_linear_desc& d = *descs[l];
     ListsLayer& L = mp.layer[l];
@@ -910,8 +979,11 @@ int gemv_lists_launch(int n, const vptq_linear_desc* const* descs, const void* x
     L.ncta = share[l];
     L.yacc = reinterpret_cast<unsigned long long*>(wsb + part_off);
     L.counters = reinterpret_cast<uint32_t*>(wsb + ctr_off);
+    L.cls = reinterpret_cast<uint16_t*>(wsb + cls_off);
+    L.lim = std::ldexp(1.f, 33 - lg_q);
     part_off += size_t(Ro[l]) * 64;
     ctr_off += size_t((Ro[l] + kRB - 1) / kRB) * 4;
+    cls_off += size_t((Ro[l] + 1) / 2) * 4;  // whole words per layer: a record word never spans two layers
     mp.grid_begin[l] = begin;
     begin += uint32_t(share[l]);
   }
