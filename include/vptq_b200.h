@@ -245,6 +245,16 @@ VPTQ_B200_API int vptq_b200_quant_gemv_multi_ws(int32_t n, const vptq_linear_des
  * sets *error (the outputs of that token are then undefined; later waits return at once): the host must check
  * it.  No reference counterpart.
  *
+ * Checked before any descriptor (VPTQ_ERR_INVALID): 0 <= slot < num_slots and -1 <= wait_slot < num_slots for both
+ * formats (epoch, done and the flag arrays hold num_slots entries); VPTQ_TP_TAGGED: ys[l] and every non-NULL
+ * peer_y[l][r] 16-byte aligned; VPTQ_TP_PLAIN: every non-NULL peer_y[l][r] at the same address modulo 16 bytes as
+ * ys[l] (the kernels store 16-byte vectors to peer_y[l][r] + o wherever ys[l] + o is aligned).
+ * world == 1 is an exchange like any other: the launch stores its tagged words (into peer_y[l][0]), advances its
+ * epochs and is refused on the generic route in the tagged format exactly as rank 0 of a larger world, so the same
+ * chain, vptq_b200_tp_untag included, runs on one GPU.
+ * The epoch counters wrap at 2^32: flag waits compare serial numbers (int32_t(flag - want) < 0), and the tags are
+ * uint32 arithmetic, so a chain may run indefinitely.
+ *
  * Two wire formats (vptq_tp_exchange::format):
  *   VPTQ_TP_PLAIN   16-bit outputs stored as they are + one epoch flag per (launch, source rank); the producer
  *                   needs two system-scope fences per launch (data before flag), ~8 us per dependent launch.
@@ -277,7 +287,7 @@ typedef struct vptq_tp_exchange {
   uint32_t* done;    /* local uint32 [num_slots], zero-initialised once */
   uint32_t* error;   /* local uint32, set to 1 when a flag wait timed out (~2 s) */
   int32_t format;    /* VPTQ_TP_PLAIN or VPTQ_TP_TAGGED */
-  int32_t num_slots; /* launches per token (tag arithmetic of VPTQ_TP_TAGGED) */
+  int32_t num_slots; /* launches per token: entries of epoch / done / the flag arrays; tag arithmetic */
 } vptq_tp_exchange;
 
 VPTQ_B200_API int vptq_b200_quant_gemv_multi_tp(int32_t n, const vptq_linear_desc* const* descs, const void* x,

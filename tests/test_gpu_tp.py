@@ -97,9 +97,9 @@ def _worker_p2p(rank, world, port, q):
         error = torch.zeros(1, dtype=torch.int32, device=dev)
         locA, locB = 2048 // world, 1024 // world
         exA = tp.make_exchange(arena, slot=0, wait_slot=-1, y_offsets=[offA], slice_bytes=[rank * locA * 2],
-                               flags_offset=off_flags, epoch=epoch, done=done, error=error)
+                               flags_offset=off_flags, epoch=epoch, done=done, error=error, num_slots=2)
         exB = tp.make_exchange(arena, slot=1, wait_slot=0, y_offsets=[offB], slice_bytes=[rank * locB * 2],
-                               flags_offset=off_flags, epoch=epoch, done=done, error=error)
+                               flags_offset=off_flags, epoch=epoch, done=done, error=error, num_slots=2)
         fA = native.FusedGemvTP([shards[0]._desc_cache[0]], [yA[:, rank * locA:(rank + 1) * locA]], exA)
         fB = native.FusedGemvTP([shards[1]._desc_cache[0]], [yB[:, rank * locB:(rank + 1) * locB]], exB)
         errs = []

@@ -274,6 +274,41 @@ int vptq_b200_quant_gemv_multi_tp(int32_t n, const vptq_linear_desc* const* desc
               tp->world, tp->rank, tp->slot);
     return VPTQ_ERR_INVALID;
   }
+  // The exchange itself, before any descriptor: a slot outside the epoch / flag arrays or a store the kernel would
+  // issue to a misaligned peer address must never reach a launch.
+  if (tp->num_slots <= tp->slot || tp->wait_slot < -1 || tp->wait_slot >= tp->num_slots) {
+    set_error("quant_gemv_multi_tp: need 0 <= slot < num_slots and -1 <= wait_slot < num_slots (slot %d, wait_slot "
+              "%d, num_slots %d)", tp->slot, tp->wait_slot, tp->num_slots);
+    return VPTQ_ERR_INVALID;
+  }
+  if (n > VPTQ_MAX_FUSED) {
+    set_error("quant_gemv_multi_tp: %d layers exceed VPTQ_MAX_FUSED (%d)", n, VPTQ_MAX_FUSED);
+    return VPTQ_ERR_INVALID;
+  }
+  const bool tagged = tp->format == VPTQ_TP_TAGGED;
+  for (int l = 0; l < n; ++l) {
+    const uintptr_t y = reinterpret_cast<uintptr_t>(ys[l]);
+    if (!y) {
+      set_error("quant_gemv_multi_tp: ys[%d] is NULL", l);
+      return VPTQ_ERR_INVALID;
+    }
+    if (tagged && (y & 15u)) {
+      set_error("quant_gemv_multi_tp: VPTQ_TP_TAGGED needs ys[%d] 16-byte aligned", l);
+      return VPTQ_ERR_INVALID;
+    }
+    for (int r = 0; r < tp->world; ++r) {
+      const uintptr_t peer = reinterpret_cast<uintptr_t>(tp->peer_y[l][r]);
+      if (!peer) continue;  // (NULL: refused below for every rank but this one)
+      if (tagged && (peer & 15u)) {
+        set_error("quant_gemv_multi_tp: VPTQ_TP_TAGGED needs peer_y[%d][%d] 16-byte aligned", l, r);
+        return VPTQ_ERR_INVALID;
+      }
+      if (!tagged && ((peer - y) & 15u)) {
+        set_error("quant_gemv_multi_tp: peer_y[%d][%d] - ys[%d] must be a multiple of 16 bytes", l, r, l);
+        return VPTQ_ERR_INVALID;
+      }
+    }
+  }
   for (int l = 0; l < n; ++l) {
     if (int rc = validate(descs[l], l == 0)) return rc;
     if (!ys[l] || y_strides[l] < descs[l]->out_features || x_stride < descs[l]->in_features) {

@@ -413,7 +413,7 @@ int gemv_multi_launch(int n, const vptq_linear_desc* const* descs, const void* x
       if (rc != VPTQ_ERR_UNSUPPORTED && rc != VPTQ_ERR_WORKSPACE) return rc;
     }
   }
-  if (tp && tp->world > 1 && tp->format == VPTQ_TP_TAGGED) {
+  if (tp && tp->format == VPTQ_TP_TAGGED) {
     set_error("gemv_multi: the tagged exchange format is implemented by the list kernel only (layers without index "
               "lists, several tokens or no workspace: use VPTQ_TP_PLAIN)");
     return VPTQ_ERR_UNSUPPORTED;
@@ -480,7 +480,7 @@ int gemv_multi_launch(int n, const vptq_linear_desc* const* descs, const void* x
     fill_params(mp.layer[l], *descs[l], pl, x_stride, y_strides[l], nullptr);
     mp.layer[l].x = x;
     mp.layer[l].y = ys[l];
-    if (tp && tp->world > 1) {
+    if (tp) {
       GemvParams& q = mp.layer[l];
       q.tp_world = tp->world, q.tp_rank = tp->rank, q.tp_slot = tp->slot, q.tp_wait_slot = tp->wait_slot;
       for (int r = 0; r < tp->world; ++r) q.tp_peer_y[r] = tp->peer_y[l][r], q.tp_peer_flags[r] = tp->peer_flags[r];

@@ -57,8 +57,8 @@ struct GemvParams {
   int I, O, Ro, G, gs, S, vol, Kol, Rol;
   int K, Kr, ib, rb;
   int idx_tma_ok;  // rows are 16-byte aligned -> bulk copies legal
-  // tensor-parallel exchange over peer memory (tp_world <= 1: off).  The kernel stores every output
-  // value into the same slot of every rank's full-width y (NVLink stores), the last CTA to finish
+  // tensor-parallel exchange over peer memory (tp_world == 0: off; world 1 still publishes epochs).  The kernel stores
+  // every output value into the same slot of every rank's full-width y (NVLink stores), the last CTA to finish
   // publishes a per-launch epoch flag on every peer, and the consumer launch polls those flags
   // before it reads x: no memset, no NCCL call, no extra kernel between two layers.
   int tp_world, tp_rank, tp_slot, tp_wait_slot;
@@ -355,7 +355,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
   stamp(4);
   // -------- phase B: x arrives from the previous kernel ------------------------------------
   pdl_wait_prior_grid();
-  if (p.tp_world > 1 && p.tp_wait_slot >= 0) {
+  if (p.tp_world > 0 && p.tp_wait_slot >= 0) {
     // x is assembled from every rank's slice: wait until all peers have published the epoch of the
     // launch that produces it (this launch's own run number: both run once per token)
     if (tid == 0) {
@@ -364,7 +364,9 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
       const long long t0 = clock64();
       for (int r = 0; r < p.tp_world; ++r) {
         if (r == p.tp_rank) continue;
-        while (ld_acquire_sys_u32(mine + r) < want) {
+        // (serial-number compare: correct across the wrap of the 32-bit epoch)
+        while (int32_t(ld_acquire_sys_u32(mine + r) - want) < 0) {
+          if (ld_volatile_u32(p.tp_error) != 0u) break;  // an earlier wait timed out: the token is lost anyway
           if (clock64() - t0 > (1ll << 32)) {  // ~2 s: give up loudly instead of hanging the GPU
             *p.tp_error = 1u;
             break;
@@ -441,7 +443,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
     const T hv = DT<T>::from_float(v);
     const int64_t off = int64_t(t) * p.y_stride + o;
     y[off] = hv;
-    if (p.tp_world > 1) {
+    if (p.tp_world > 0) {
       stored_to_peers = true;
 #pragma unroll 1
       for (int r = 0; r < p.tp_world; ++r)
@@ -654,7 +656,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
           const uint4 pk = make_uint4(DT<T>::pack2(v[0], v[1]), DT<T>::pack2(v[2], v[3]), DT<T>::pack2(v[4], v[5]),
                                       DT<T>::pack2(v[6], v[7]));
           *reinterpret_cast<uint4*>(y + off) = pk;
-          if (p.tp_world > 1) {
+          if (p.tp_world > 0) {
             stored_to_peers = true;
 #pragma unroll 1
             for (int r = 0; r < p.tp_world; ++r)
@@ -681,7 +683,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
   }
 
   // -------- tensor-parallel hand-off: publish this launch's epoch on every peer ------------------
-  if (p.tp_world > 1) {
+  if (p.tp_world > 0) {
     if (stored_to_peers) __threadfence_system();  // this thread's peer stores are visible system-wide
     __syncthreads();
     if (tid == 0) {

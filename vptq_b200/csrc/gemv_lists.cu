@@ -103,7 +103,7 @@ struct ListsParams {
   uint32_t off_bars, off_tab, off_red, off_piece, off_done, off_slice, off_res, off_x, off_ring;
   int stages;
   unsigned long long* prof;  // developer aid: %globaltimer stamps of the first / last CTA (or nullptr)
-  // tensor-parallel exchange over peer memory (tp_world <= 1: off), same protocol as the generic kernel
+  // tensor-parallel exchange over peer memory (tp_world == 0: off), same protocol as the generic kernel
   // (gemv_kernel.cuh): every output row is stored locally and into all peers' buffers, the last CTA of the
   // launch publishes the launch's epoch in every peer's flag array, a launch with tp_wait_slot >= 0 polls the
   // flags of the launch that produced its x before reading it
@@ -389,12 +389,12 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
   }
   // -------- x arrives from the previous kernel: one coalesced 128-bit load per thread ---------------------------
   pdl_wait_prior_grid();
-  const bool tagged = mp.tp_world > 1 && mp.tp_format == VPTQ_TP_TAGGED;
+  const bool tagged = mp.tp_world > 0 && mp.tp_format == VPTQ_TP_TAGGED;
   // tag of the words this launch writes / expects in its x: run number * launches per token + slot + 1
-  const uint32_t run = mp.tp_world > 1 ? ld_volatile_u32(mp.tp_epoch + mp.tp_slot) : 0u;
+  const uint32_t run = mp.tp_world > 0 ? ld_volatile_u32(mp.tp_epoch + mp.tp_slot) : 0u;
   const uint32_t tag_out = run * uint32_t(mp.tp_nslots) + uint32_t(mp.tp_slot) + 1u;
   const uint32_t tag_in = run * uint32_t(mp.tp_nslots) + uint32_t(mp.tp_wait_slot) + 1u;
-  if (mp.tp_world > 1 && mp.tp_wait_slot >= 0 && !tagged) {
+  if (mp.tp_world > 0 && mp.tp_wait_slot >= 0 && !tagged) {
     // x is assembled from every rank's slice: wait until all peers have published the epoch of the launch
     // that produces it (= this launch's own run number: both run once per token).  A wait that times out
     // (~2 s) sets the error word, which the host checks; once it is set nobody waits any more.
@@ -402,7 +402,7 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
       const uint32_t want = run + 1u;
       const uint32_t* flag = mp.tp_peer_flags[mp.tp_rank] + mp.tp_wait_slot * mp.tp_world + tid;
       const long long t0 = clock64();
-      while (ld_acquire_sys_u32(flag) < want) {
+      while (int32_t(ld_acquire_sys_u32(flag) - want) < 0) {  // (serial-number compare: wrap-safe)
         if (ld_volatile_u32(mp.tp_error) != 0u) break;
         if (clock64() - t0 > (1ll << 32)) {
           *mp.tp_error = 1u;
@@ -718,7 +718,7 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
                            "r"(pk.w), "r"(tag_out)
                            : "memory");
             }
-          } else if (mp.tp_world > 1) {
+          } else if (mp.tp_world > 0) {
             for (int rk = 0; rk < mp.tp_world; ++rk)
               if (rk != mp.tp_rank) *reinterpret_cast<uint4*>(reinterpret_cast<T*>(mp.tp_peer_y[l][rk]) + o) = pk;
             stored_to_peers = true;
@@ -729,7 +729,7 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
             if (o + e < L.O) {
               const T hv = DT<T>::from_float(v[e]);
               y[o + e] = hv;
-              if (mp.tp_world > 1 && !tagged) {
+              if (mp.tp_world > 0 && !tagged) {
                 for (int rk = 0; rk < mp.tp_world; ++rk)
                   if (rk != mp.tp_rank) reinterpret_cast<T*>(mp.tp_peer_y[l][rk])[o + e] = hv;
                 stored_to_peers = true;
@@ -742,7 +742,7 @@ __global__ void __launch_bounds__(kLT, 1) gemv_lists_kernel(const __grid_constan
     if (tid < nd) L.counters[s_done[tid]] = 0u;  // leave the counters zeroed for the next launch
   }
   // -------- tensor-parallel hand-off: the last CTA of the launch publishes its epoch on every peer ----------
-  if (mp.tp_world > 1) {
+  if (mp.tp_world > 0) {
     if (stored_to_peers) __threadfence_system();  // this thread's peer stores are visible system-wide
     __syncthreads();
     if (tid == 0) {
@@ -988,7 +988,7 @@ int gemv_lists_launch(int n, const vptq_linear_desc* const* descs, const void* x
     begin += uint32_t(share[l]);
   }
   for (int l = n; l <= kMaxFusedLayers; ++l) mp.grid_begin[l] = begin;
-  if (tp && tp->world > 1) {
+  if (tp) {  // (world 1 included: the same stores, tags and epochs as rank 0 of a larger world)
     mp.tp_world = tp->world, mp.tp_rank = tp->rank, mp.tp_slot = tp->slot, mp.tp_wait_slot = tp->wait_slot;
     for (int l = 0; l < n; ++l)
       for (int r = 0; r < tp->world; ++r) mp.tp_peer_y[l][r] = tp->peer_y[l][r];

@@ -386,7 +386,7 @@ class FusedGemvTP:
             if self.ws_bytes is None:
                 self.ws_bytes = sum(workspace_bytes(d, x2d.shape[0], OP_GEMV) for d in self.descs)
             ws = workspace(dev, self.ws_bytes)
-            rc = lib().vptq_b200_quant_gemv_multi_tp(self.n, self.desc_arr, x2d.data_ptr(), x2d.stride(0), self.y_arr,
+            rc = lib().vptq_b200_quant_gemv_multi_tp(self.n, self.desc_arr, x2d.data_ptr(), row_pitch(x2d), self.y_arr,
                                                      self.stride_arr, x2d.shape[0], ctypes.byref(self.ex), ws.data_ptr(),
                                                      ws.numel(), flags, _stream(dev))
         check(rc, "vptq_b200_quant_gemv_multi_tp")

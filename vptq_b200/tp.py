@@ -181,10 +181,11 @@ class PeerArena:
 
 
 def make_exchange(arena: PeerArena, *, slot: int, wait_slot: int, y_offsets, slice_bytes, flags_offset: int,
-                  epoch: torch.Tensor, done: torch.Tensor, error: torch.Tensor, fmt: int = 0, num_slots: int = 0):
+                  epoch: torch.Tensor, done: torch.Tensor, error: torch.Tensor, num_slots: int, fmt: int = 0):
     """Fill a vptq_tp_exchange for one launch: y_offsets[l] = byte offset (in the arena) of layer l's FULL-width
-    output buffer, slice_bytes[l] = byte offset of this rank's slice inside it.  fmt = native.TP_TAGGED: the
-    buffers are tagged-word buffers (4 bytes per output, include/vptq_b200.h) and num_slots = launches per token."""
+    output buffer, slice_bytes[l] = byte offset of this rank's slice inside it, num_slots = launches per token (the
+    length of `epoch`, `done` and the flag array; the library refuses slot or wait_slot outside it).
+    fmt = native.TP_TAGGED: the buffers are tagged-word buffers (4 bytes per output, include/vptq_b200.h)."""
     from . import native
     ex = native.TpExchange()
     import ctypes
