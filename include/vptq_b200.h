@@ -89,7 +89,7 @@ typedef struct vptq_linear_desc {
   int32_t out_features;          /* O                                                        */
   int32_t vector_len;            /* v   = vector_lens[1]   (even, 2..16)                     */
   int32_t num_centroids;         /* K   = num_centroids[1] (power of two, <= 65536)          */
-  int32_t num_res_centroids;     /* Kr  (power of two; <= 0: no residual codebook)           */
+  int32_t num_res_centroids;     /* Kr  (power of two >= 2; <= 0: no residual codebook)      */
   int32_t num_codebooks;         /* G   = group_num                                          */
   int32_t group_size;            /* gs  columns per codebook group; S + G*gs == I            */
   int32_t outlier_size;          /* S   leading outlier columns (0: none)                    */

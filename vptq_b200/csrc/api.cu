@@ -87,8 +87,11 @@ int validate(const vptq_linear_desc* d, bool need_device) {
     set_error("num_centroids %d must be a power of two in [2,65536]", d->num_centroids);
     return VPTQ_ERR_UNSUPPORTED;
   }
-  if (d->num_res_centroids > 0 && (!is_pow2(d->num_res_centroids) || d->num_res_centroids > 65536)) {
-    set_error("num_res_centroids %d must be a power of two <= 65536", d->num_res_centroids);
+  // (a single residual entry would need 0 index bits: the packed format cannot tell it from "no residual", so it is
+  // refused rather than added to some weights and not to others)
+  if (d->num_res_centroids > 0 &&
+      (!is_pow2(d->num_res_centroids) || d->num_res_centroids > 65536 || d->num_res_centroids < 2)) {
+    set_error("num_res_centroids %d must be a power of two in [2,65536] (or <= 0: no residual)", d->num_res_centroids);
     return VPTQ_ERR_UNSUPPORTED;
   }
   const int ib = ilog2(d->num_centroids);

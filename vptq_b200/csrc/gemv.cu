@@ -45,10 +45,10 @@ const Tune& tune() {
   return t;
 }
 
-GemvKernelFn pick_kernel(const vptq_linear_desc& d, int nt, bool main_smem) {
+GemvKernelFn pick_kernel(const vptq_linear_desc& d, int nt, bool main_smem, bool res_smem) {
   const bool res = d.num_res_centroids > 0;
-  return d.vector_len == 8 ? gemv_kernel_v8(d.dtype, nt, main_smem, res)
-                           : gemv_kernel_vx(d.dtype, d.vector_len, main_smem, res);
+  return d.vector_len == 8 ? gemv_kernel_v8(d.dtype, nt, main_smem, res, !res_smem)
+                           : gemv_kernel_vx(d.dtype, d.vector_len, main_smem, res, !res_smem);
 }
 
 }  // namespace
@@ -135,19 +135,24 @@ int gemv_make_plan(const vptq_linear_desc& d, int tokens, const DeviceInfo& dev,
   // gives every layer its share of the SMs
   const int slots = slots_override > 0 ? std::min(slots_override, sms) : sms;
 
-  // One attempt = (warps per CTA, main codebook in shared memory?).  First fit wins.
-  struct Attempt { int warps; bool main_smem; };
-  const Attempt attempts[] = {{16, true}, {8, true}, {16, false}, {8, false}};
+  // One attempt = (warps per CTA, main codebook in shared memory?, residual codebook in shared memory?).  First fit
+  // wins.  A residual codebook is gathered through L1/L2 only when no layout with it in shared memory fits (256 KiB
+  // and up, e.g. Kr = 65536 at any v): the last four attempts, planned with res_rep = 0.
+  struct Attempt { int warps; bool main_smem; bool res_smem; };
+  const Attempt attempts[] = {{16, true, true},   {8, true, true},   {16, false, true},  {8, false, true},
+                              {16, true, false},  {8, true, false},  {16, false, false}, {8, false, false}};
   for (const Attempt& a : attempts) {
     if (a.main_smem && !main_fits) continue;
+    if (!a.res_smem && !rb) continue;
     if (tn.warps && a.warps != tn.warps) continue;
+    const size_t res_smem_bytes = a.res_smem ? res_bytes : 0;
 
     // ---- column chunks (cpg per codebook group, multiples of 128 columns) x warps per row -------
     // A CTA streams rows_cta * cc fields; its nwarps/wsplit row slots work in parallel, each row
     // cut over wsplit warps.  Chunk counts up to 8 reduce through a cluster (the co-schedulable
     // cluster count can leave SMs idle: a cluster must fit inside one GPC), more than 8
     // through global memory.
-    GemvKernelFn fn_probe = pick_kernel(d, pl.nt, a.main_smem);
+    GemvKernelFn fn_probe = pick_kernel(d, pl.nt, a.main_smem, a.res_smem);
     int best_cpg = 0, best_cc = 0, best_ws = 1;
     double best_cost = 1e300;
     for (int cpg = 1; cpg <= 64; cpg *= 2) {
@@ -220,11 +225,11 @@ int gemv_make_plan(const vptq_linear_desc& d, int tokens, const DeviceInfo& dev,
       pl.off_wcnt = uint32_t(off);
       if (pl.wsplit > 1) off += align_up(size_t(rows_alloc) * 4, 128);
       pl.off_res = uint32_t(off);
-      off += align_up(res_bytes * res_rep, 128);
+      off += align_up(res_smem_bytes * res_rep, 128);
       pl.off_main = uint32_t(off);
       if (a.main_smem) off += align_up(main_bytes * pl.main_rep, 128);
       pl.off_raw = uint32_t(off);
-      off += align_up((res_rep > 1 ? res_bytes : 0) + (a.main_smem && pl.main_rep > 1 ? main_bytes : 0), 128);
+      off += align_up((res_rep > 1 ? res_smem_bytes : 0) + (a.main_smem && pl.main_rep > 1 ? main_bytes : 0), 128);
       pl.off_ring = uint32_t(off);
       off += align_up(size_t(warps) * stages * pl.stage_bytes, 128);
       return off;
@@ -235,7 +240,7 @@ int gemv_make_plan(const vptq_linear_desc& d, int tokens, const DeviceInfo& dev,
     struct Shape { int stages, rep; };
     std::vector<Shape> shapes;
     for (int st : (a.main_smem ? std::vector<int>{4, 3, 2} : std::vector<int>{2}))
-      for (int rep : {res_rep_max, 1}) shapes.push_back({st, rep});
+      for (int rep : {a.res_smem ? res_rep_max : 0, a.res_smem ? 1 : 0}) shapes.push_back({st, rep});
     bool placed = false;
     for (const Shape& sh : shapes) {
       if (tn.stages && sh.stages != tn.stages) continue;
@@ -376,7 +381,7 @@ int gemv_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void
   for (int t0 = 0; t0 < tokens;) {
     int nt = pl.nt;
     while (nt > tokens - t0) nt >>= 1;  // tail passes: 4 -> 2 -> 1
-    GemvKernelFn fn = pick_kernel(d, nt, pl.main_in_smem != 0);
+    GemvKernelFn fn = pick_kernel(d, nt, pl.main_in_smem != 0, pl.res_rep > 0);
     if (!fn) {
       set_error("gemv: no kernel for dtype=%d v=%d nt=%d", d.dtype, d.vector_len, nt);
       return VPTQ_ERR_UNSUPPORTED;
@@ -447,7 +452,8 @@ int gemv_multi_launch(int n, const vptq_linear_desc* const* descs, const void* x
   // 2. SMs that can be used at once: all clusters of all layers must be co-resident
   int avail = dev->sm_count;
   if (plans[big].cluster) {
-    GemvKernelFn probe = pick_kernel(*descs[big], plans[big].nt, plans[big].main_in_smem != 0);
+    GemvKernelFn probe = pick_kernel(*descs[big], plans[big].nt, plans[big].main_in_smem != 0,
+                                     plans[big].res_rep > 0);
     const int nmax = probe ? max_active_clusters(reinterpret_cast<const void*>(probe), nch, plans[big].threads,
                                                  200 * 1024, dev->smem_optin)
                            : -1;
@@ -473,7 +479,8 @@ int gemv_multi_launch(int n, const vptq_linear_desc* const* descs, const void* x
   for (int l = 0; l < n; ++l) {
     const GemvPlan& pl = plans[l];
     if (pl.nch != plans[big].nch || pl.threads != plans[big].threads || pl.cluster != plans[big].cluster ||
-        pl.main_in_smem != plans[big].main_in_smem || pl.nt != plans[big].nt || pl.ws_partials_bytes) {
+        pl.main_in_smem != plans[big].main_in_smem || (pl.res_rep > 0) != (plans[big].res_rep > 0) ||
+        pl.nt != plans[big].nt || pl.ws_partials_bytes) {
       set_error("gemv_multi: the layers do not admit one launch configuration");
       return VPTQ_ERR_UNSUPPORTED;
     }
@@ -491,7 +498,8 @@ int gemv_multi_launch(int n, const vptq_linear_desc* const* descs, const void* x
     smem = std::max(smem, pl.smem_bytes);
   }
   for (int l = n; l <= kMaxFused; ++l) mp.grid_begin[l] = begin;
-  GemvMultiKernelFn fn = gemv_multi_kernel_v8(d0.dtype, plans[big].nt, plans[big].main_in_smem != 0, d0.num_res_centroids > 0);
+  GemvMultiKernelFn fn = gemv_multi_kernel_v8(d0.dtype, plans[big].nt, plans[big].main_in_smem != 0,
+                                              d0.num_res_centroids > 0, plans[big].res_rep == 0);
   if (!fn || plans[big].nt != tokens) {
     set_error("gemv_multi: no fused kernel for this configuration");
     return VPTQ_ERR_UNSUPPORTED;

@@ -125,9 +125,13 @@ __device__ __forceinline__ float warp_reduce_to_lane(float (&acc)[V], int lane) 
 
 // One CTA's share of one layer.  `bidx` / `gdim`: this CTA's index within, and the size of, the
 // layer's own grid (a fused launch concatenates the grids of several layers, see gemv_multi_kernel).
-template <typename T, int V, int NT, bool MAIN_SMEM, bool RES>
+// RES_L2: the residual codebook does not fit in shared memory (256 KiB and up): its entries are gathered
+// through L1/L2 next to the main entry of the same field, like an L2-gather main codebook.
+template <typename T, int V, int NT, bool MAIN_SMEM, bool RES, bool RES_L2 = false>
 __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, const uint32_t bidx, const uint32_t gdim,
                                           const uint32_t gdim_total) {
+  static_assert(RES || !RES_L2, "RES_L2 needs a residual codebook");
+  constexpr bool RES_SMEM = RES && !RES_L2;
   constexpr int U = (NT == 1 && V <= 8) ? 8 : 4;  // independent codebook gathers in flight per lane
   constexpr int EB = 2 * V;                       // bytes per codebook entry
   const GemvPlan& pl = p.plan;
@@ -296,7 +300,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
       }
     }
   };
-  if constexpr (RES) stage_table(s_res, res_g, p.Kr, pl.res_rep, raw_res, tma_res);
+  if constexpr (RES_SMEM) stage_table(s_res, res_g, p.Kr, pl.res_rep, raw_res, tma_res);
   if constexpr (MAIN_SMEM) stage_table(s_main, cent_g, p.K, pl.main_rep, raw_main, tma_main);
   if (tid == 0) {
     if (cb_tx) mbar_arrive_expect_tx(cb_bar, cb_tx);
@@ -314,6 +318,14 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
       const uint32_t slice = ((total_b + gdim - 1) / gdim + 15u) & ~15u;
       const uint32_t off = bidx * slice;
       if (off < total_b) l2_prefetch_bulk(reinterpret_cast<const uint8_t*>(cent_g) + off, min(slice, total_b - off));
+    }
+  }
+  if constexpr (RES_L2) {
+    if (tid == 64) {
+      const uint32_t total_b = uint32_t(p.Kr) * EB;
+      const uint32_t slice = ((total_b + gdim - 1) / gdim + 15u) & ~15u;
+      const uint32_t off = bidx * slice;
+      if (off < total_b) l2_prefetch_bulk(reinterpret_cast<const uint8_t*>(res_g) + off, min(slice, total_b - off));
     }
   }
   for (int i0 = tid; i0 < n_all; i0 += 4 * blockDim.x) {
@@ -338,7 +350,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
 
   stamp(3);
   // replicate TMA-landed tables (smem -> smem) once they have arrived
-  if constexpr (RES || MAIN_SMEM) mbar_wait(cb_bar, 0);
+  if constexpr (RES_SMEM || MAIN_SMEM) mbar_wait(cb_bar, 0);
   if constexpr (V == 8) {
     auto replicate = [&](uint8_t* dst, uint32_t raw_at, int entries) {
       const uint32_t src = smem_u32(s_raw + raw_at), d = smem_u32(dst);
@@ -348,7 +360,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
         for (int c = 0; c < 8; ++c) sts_v4(d + (e * 8 + c) * 16, v);
       }
     };
-    if (RES && tma_res && pl.res_rep > 1) replicate(s_res, raw_res, p.Kr);
+    if (RES_SMEM && tma_res && pl.res_rep > 1) replicate(s_res, raw_res, p.Kr);
     if (MAIN_SMEM && tma_main && pl.main_rep > 1) replicate(s_main, raw_main, p.K);
   }
 
@@ -576,11 +588,13 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
     const int NG = nunits * ngu;                        // (padding groups decode to field 0, no FMA)
     uint32_t fld[U];
     uint32_t cw[U][V / 2];
+    uint32_t rg[RES_L2 ? U : 1][V / 2];  // RES_L2: the residual entries, gathered with the main ones
+    const uint8_t* res_bytes = reinterpret_cast<const uint8_t*>(res_g);
     // load side: position of the next group to fetch
     int l_gl = 0, l_st = 0, l_nf = 0;
     uint32_t l_par = 0;
     const uint32_t* l_sw = reinterpret_cast<const uint32_t*>(ring);
-    auto load = [&](uint32_t& f_out, uint32_t (&c_out)[V / 2]) {
+    auto load = [&](uint32_t& f_out, uint32_t (&c_out)[V / 2], uint32_t (&r_out)[V / 2]) {
       const int gs_ = l_gl & (gps - 1);
       if (gs_ == 0) {  // first group of a ring segment: wait for its TMA, once
         mbar_wait(&full[l_st], l_par);
@@ -592,6 +606,7 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
       const uint32_t mi = f & imask;
       if constexpr (MAIN_SMEM) lds_entry<V>(c_out, s_main_lane + mi * main_stride);
       else ldg_entry<V>(c_out, cent_bytes + size_t(mi) * EB, pol_keep);
+      if constexpr (RES_L2) ldg_entry<V>(r_out, res_bytes + size_t(f >> p.ib) * EB, pol_keep);
       ++l_gl;
       if (l_gl == ngu || (l_gl & (gps - 1)) == 0) {  // next group starts a new segment (and maybe a new row)
         if (++l_st == pl.stages) l_st = 0, l_par ^= 1u;
@@ -602,20 +617,24 @@ __device__ __forceinline__ void gemv_body(const GemvParams& p, uint8_t* smem, co
     int c_gl = 0, c_u = 0, c_q = 0;
 #pragma unroll
     for (int k = 0; k < U; ++k)
-      if (k < NG) load(fld[k], cw[k]);
+      if (k < NG) load(fld[k], cw[k], rg[RES_L2 ? k : 0]);
     for (int n0 = 0; n0 < NG; n0 += U) {
 #pragma unroll
       for (int k = 0; k < U; ++k) {
         const int j = (c_gl + k) * 32 + lane;  // this lane's field, relative to the warp's sub-range
         uint32_t rw[V / 2];
-        if constexpr (RES) lds_entry<V>(rw, s_res_lane + (fld[k] >> p.ib) * res_stride);
+        if constexpr (RES_SMEM) lds_entry<V>(rw, s_res_lane + (fld[k] >> p.ib) * res_stride);
+        if constexpr (RES_L2) {
+#pragma unroll
+          for (int i = 0; i < V / 2; ++i) rw[i] = rg[k][i];
+        }
         // lanes past the end gathered entry 0 of both codebooks: they add nothing (not even 0 * entry, which an
         // inf or NaN there would turn into NaN in rows that never use the entry)
         if (j < wcols) {
 #pragma unroll
           for (int t = 0; t < NT; ++t) fma_entry<T, V, RES>(acc[t], sx[t * pl.sx_stride + sf0 + j], cw[k], rw);
         }
-        if (n0 + k + U < NG) load(fld[k], cw[k]);  // refill the slot: group n0+k+U
+        if (n0 + k + U < NG) load(fld[k], cw[k], rg[RES_L2 ? k : 0]);  // refill the slot: group n0+k+U
       }
       c_gl += U;
       const bool unit_done = c_gl == ngu;
@@ -707,6 +726,13 @@ __global__ void __launch_bounds__(512, 1) gemv_kernel(const __grid_constant__ Ge
   gemv_body<T, V, NT, MAIN_SMEM, RES>(p, smem, blockIdx.x, gridDim.x, gridDim.x);
 }
 
+// the same for a residual codebook too large for shared memory (planned with GemvPlan::res_rep == 0)
+template <typename T, int V, int NT, bool MAIN_SMEM>
+__global__ void __launch_bounds__(512, 1) gemv_kernel_res_l2(const __grid_constant__ GemvParams p) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  gemv_body<T, V, NT, MAIN_SMEM, true, true>(p, smem, blockIdx.x, gridDim.x, gridDim.x);
+}
+
 // Horizontal fusion: up to 4 layers that read the SAME x (q/k/v, gate/up) in ONE launch.  The grid is
 // the concatenation of the layers' own grids (each planned for its share of the SMs); a CTA finds
 // its layer from blockIdx.x and then runs the ordinary per-layer body.  One launch, one prologue
@@ -729,11 +755,23 @@ __global__ void __launch_bounds__(512, 1) gemv_multi_kernel(const __grid_constan
                                      mp.grid_begin[l + 1] - mp.grid_begin[l], gridDim.x);
 }
 
+template <typename T, int V, int NT, bool MAIN_SMEM>
+__global__ void __launch_bounds__(512, 1) gemv_multi_kernel_res_l2(const __grid_constant__ GemvMultiParams mp) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  int l = 0;
+#pragma unroll
+  for (int i = 1; i < kMaxFused; ++i)
+    if (i < mp.n && blockIdx.x >= mp.grid_begin[i]) l = i;
+  gemv_body<T, V, NT, MAIN_SMEM, true, true>(mp.layer[l], smem, blockIdx.x - mp.grid_begin[l],
+                                             mp.grid_begin[l + 1] - mp.grid_begin[l], gridDim.x);
+}
+
 using GemvKernelFn = void (*)(const GemvParams);
 using GemvMultiKernelFn = void (*)(const GemvMultiParams);
-// one definition per (dtype, V) translation unit, see gemv_inst_*.cu
-GemvKernelFn gemv_kernel_v8(int dtype, int nt, bool main_smem, bool res);
-GemvKernelFn gemv_kernel_vx(int dtype, int v, bool main_smem, bool res);
-GemvMultiKernelFn gemv_multi_kernel_v8(int dtype, int nt, bool main_smem, bool res);
+// one definition per (dtype, V) translation unit, see gemv_inst_*.cu.  res_l2 (with res): the residual codebook is
+// gathered through L1/L2 instead of shared memory
+GemvKernelFn gemv_kernel_v8(int dtype, int nt, bool main_smem, bool res, bool res_l2 = false);
+GemvKernelFn gemv_kernel_vx(int dtype, int v, bool main_smem, bool res, bool res_l2 = false);
+GemvMultiKernelFn gemv_multi_kernel_v8(int dtype, int nt, bool main_smem, bool res, bool res_l2 = false);
 
 }  // namespace vptq_b200

@@ -56,7 +56,7 @@ struct GemvPlan {
   int stages;          // ring depth per warp
   int main_in_smem;    // main codebook staged in shared memory (else gathered through L1/L2)
   int main_rep;        // bank-group replication factor of the main codebook in smem (1 or 8)
-  int res_rep;         // same for the residual codebook
+  int res_rep;         // same for the residual codebook; 0: not in shared memory, gathered through L1/L2
   int nt;              // tokens per pass (1, 2 or 4)
   int sx_stride;       // floats per token row of x' in smem
   int cluster;         // 1: the nch CTAs of a row set form a thread-block cluster (DSMEM split-K)

@@ -91,6 +91,9 @@ class VQuantLinear(nn.Module):
         self.indices_as_float = indices_as_float
         self.is_indice_packed = is_indice_packed
         self.enable_norm, self.enable_perm = enable_norm, enable_perm
+        if self.num_res_centroids == 1:
+            # 0 index bits: the packed format has no field that could tell one residual entry from none
+            raise ValueError("num_res_centroids = 1 is not supported: use -1 (no residual) or a power of two >= 2")
         self.enable_residual = self.num_res_centroids > 0
         self.enable_outlier = bool(self.outlier_vector_len > 1 and self.num_outlier_centroids > 0)
         self.padding = (-out_features) % self.vector_len

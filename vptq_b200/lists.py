@@ -62,6 +62,13 @@ def eligible(*, vector_len: int, num_centroids: int, num_res_centroids: int, num
             and 8 <= in_features <= 65535)
 
 
+def launchable(in_features: int, num_centroids: int, sm_count: int) -> bool:
+    """The list kernel gives every (slice, tile) combo at least one CTA of a one-CTA-per-SM grid: a layer whose
+    NS * NT exceeds the SM count never runs on it (gemv_lists_launch), so its lists are not worth building."""
+    ns, nt, _ = geometry(in_features, num_centroids)
+    return ns * nt <= int(sm_count)
+
+
 DEAL_DEFAULT = "1"   # VPTQ_B200_LISTS_DEAL when unset
 
 

@@ -186,6 +186,16 @@ def require_cuda(name: str, t: Optional[torch.Tensor], contiguous: bool = True) 
         raise RuntimeError(f"{name} must be contiguous")
 
 
+_sm_counts: dict = {}
+
+
+def _sm_count(device: torch.device) -> int:
+    idx = device.index if device.index is not None else torch.cuda.current_device()
+    if idx not in _sm_counts:
+        _sm_counts[idx] = torch.cuda.get_device_properties(idx).multi_processor_count
+    return _sm_counts[idx]
+
+
 def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector_len: int, num_centroids: int,
               num_res_centroids: int, num_codebooks: int, group_size: int, outlier_size: int,
               outlier_vector_len: int, num_outlier_centroids: int, indices: torch.Tensor,
@@ -251,7 +261,8 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
     if lists and derive and _lists.eligible(
             vector_len=d.vector_len, num_centroids=d.num_centroids, num_res_centroids=d.num_res_centroids,
             num_codebooks=d.num_codebooks, outlier_size=d.outlier_size, in_features=d.in_features) and (
-            weight_scale is None or (weight_scale.data_ptr() % 16 == 0 and weight_bias.data_ptr() % 16 == 0)):
+            weight_scale is None or (weight_scale.data_ptr() % 16 == 0 and weight_bias.data_ptr() % 16 == 0)) and (
+            _lists.launchable(d.in_features, d.num_centroids, _sm_count(indices.device))):
         stream, tab, tcw = _lists.build_lists(indices, num_centroids=d.num_centroids,
                                               num_res_centroids=d.num_res_centroids, in_features=d.in_features,
                                               out_features=d.out_features, perm=perm)
@@ -259,7 +270,8 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
         d._keep = d._keep + (stream, tab)
     if drop_packed:
         if not d.lists_stream:
-            raise RuntimeError("drop_packed: this layer has no index lists (not eligible, or lists=False)")
+            raise RuntimeError("drop_packed: this layer has no index lists (not eligible, its slices x column tiles "
+                               "exceed the device's SM count, or lists=False)")
         d.indices = None
     return d
 
