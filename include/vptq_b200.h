@@ -349,6 +349,8 @@ VPTQ_B200_API int vptq_b200_linear_host(const vptq_linear_desc* desc, const void
                           int32_t tokens, void* x_dev, void* y_dev, void* workspace,
                           size_t workspace_bytes, uint32_t flags, void* stream);
 
+/* Workspace helpers for hosts that capture CUDA graphs: include/vptq_b200_graph.h. */
+
 #ifdef __cplusplus
 }
 #endif

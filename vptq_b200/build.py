@@ -41,6 +41,7 @@ def _headers():
     hs = [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".cuh", ".h"))]
     hs.append(os.path.join(INCLUDE, "vptq_b200.h"))
     hs.append(os.path.join(INCLUDE, "vptq_b200_grad.h"))
+    hs.append(os.path.join(INCLUDE, "vptq_b200_graph.h"))
     return hs
 
 

@@ -491,4 +491,20 @@ int vptq_b200_linear_host(const vptq_linear_desc* desc, const void* x_host, void
   return 0;
 }
 
+int vptq_b200_stream_capture_id(void* stream, uint64_t* id) {
+  if (!id) {
+    set_error("stream_capture_id: NULL id");
+    return VPTQ_ERR_INVALID;
+  }
+  cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+  unsigned long long cid = 0;
+  cudaError_t e = cudaStreamGetCaptureInfo(static_cast<cudaStream_t>(stream), &st, &cid);
+  if (e != cudaSuccess) {
+    set_error("cudaStreamGetCaptureInfo: %s", cudaGetErrorString(e));
+    return VPTQ_ERR_CUDA;
+  }
+  *id = st == cudaStreamCaptureStatusActive ? uint64_t(cid) : 0;
+  return st == cudaStreamCaptureStatusActive ? 1 : 0;
+}
+
 }  // extern "C"

@@ -7,6 +7,7 @@
 
 #include "../../include/vptq_b200.h"
 #include "../../include/vptq_b200_grad.h"
+#include "../../include/vptq_b200_graph.h"
 
 namespace vptq_b200 {
 

@@ -32,6 +32,13 @@ __all__ = ["fuse", "unfuse", "set_quant_grad", "FusedGroup", "FusedMember", "DEF
 DEFAULT_GROUPS: Tuple[Tuple[str, ...], ...] = (("q_proj", "k_proj", "v_proj"), ("gate_proj", "up_proj"))
 
 
+def activation_key(x: torch.Tensor) -> tuple:
+    """Identity of a decode activation for FusedGroup's output cache.  An inference tensor has no version counter:
+    a write to x inside torch.inference_mode() between two members' calls goes unseen (a new activation at the same
+    address does not: each member is served once)."""
+    return (x.data_ptr(), 0 if x.is_inference() else x._version, tuple(x.shape), x.dtype, x.device)
+
+
 class FusedGroup:
     """Shared state of one sibling group (not an nn.Module: the layers stay owned by their FusedMembers)."""
 
@@ -63,7 +70,7 @@ class FusedGroup:
         tokens = x2.shape[0]
         if not x.is_cuda or tokens < 1 or tokens > 2 or x2.stride(-1) != 1 or (tokens > 1 and x2.stride(0) < x2.shape[1]):
             return None
-        key = (x.data_ptr(), x._version, tuple(x.shape), x.dtype, x.device)
+        key = activation_key(x)
         if key == self._key and self._out is not None and not (self._served >> index) & 1:
             self._served |= 1 << index
             if self._served == (1 << len(self.layers)) - 1:

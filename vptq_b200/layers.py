@@ -36,6 +36,12 @@ def _frozen(shape, dtype, device) -> Parameter:
     return Parameter(torch.empty(shape, dtype=dtype, device=device), requires_grad=False)
 
 
+def _version(t: torch.Tensor) -> int:
+    """t._version, or 0 for an inference tensor: it has no version counter (reading it raises), and writes to it are
+    only possible inside torch.inference_mode(), where the caches cannot see them (prepare(rebuild=True))."""
+    return 0 if t.is_inference() else t._version
+
+
 class VQuantLinear(nn.Module):
     """VPTQ quantized linear layer (see the module docstring for the tensors it holds).
 
@@ -167,7 +173,7 @@ class VQuantLinear(nn.Module):
     def _packed_indices(self) -> torch.Tensor:
         if self.is_indice_packed:
             return self.indices
-        key = (self.indices.data_ptr(), self.indices._version)
+        key = tuple((a.data_ptr(), _version(a)) if a is not None else None for a in (self.indices, self.res_indices))
         if self._packed is None or self._packed[0] != key:
             ib = int(math.log2(self.num_centroids))
             rb = int(math.log2(self.num_res_centroids)) if self.enable_residual else 0
@@ -176,8 +182,10 @@ class VQuantLinear(nn.Module):
         return self._packed[1]
 
     def _cache_key(self, t, dtype, device):
-        # data_ptr catches .to() / re-assignment, _version catches in-place updates (load_state_dict, copy_)
-        return tuple((a.data_ptr(), a.dtype, a._version) if a is not None else None for a in t) + (dtype, device)
+        # data_ptr catches .to() / re-assignment, _version catches in-place updates (load_state_dict, copy_);
+        # res_indices (unpacked checkpoints) is packed into the words the descriptor points to
+        return tuple((a.data_ptr(), a.dtype, _version(a)) if a is not None else None
+                     for a in t + (self.res_indices,)) + (dtype, device)
 
     # positions in _tensors() of the floating-point tensors the descriptor only points to (codebooks, scale, bias):
     # an in-place update of them (an optimizer step) keeps the descriptor and its index lists
@@ -226,14 +234,29 @@ class VQuantLinear(nn.Module):
         _, cent, resc, _, outc, _, ws, wb, _ = self._tensors()
         return any(t is not None and t.requires_grad for t in (cent, resc, outc, ws, wb))
 
-    def prepare(self, dtype: Optional[torch.dtype] = None, drop_packed: bool = False) -> "VQuantLinear":
+    def prepare(self, dtype: Optional[torch.dtype] = None, drop_packed: bool = False,
+                rebuild: bool = False) -> "VQuantLinear":
         """Build the C-ABI descriptor and its load-time derivatives (scale/bias in quantised order, the
         slice x tile index lists of the decode kernel) now instead of inside the first forward: call once
         after loading the checkpoint, before capturing CUDA graphs.
 
+        The descriptor is kept as long as the parameters' storage and version counters say nothing changed.  After an
+        in-place update of the parameters (an optimizer step, `mul_`, `copy_`), call `prepare()` again before
+        replaying a captured CUDA graph: it refreshes the quantised-order copies of weight_scale / weight_bias, which
+        only `forward` does otherwise.  Writes the version counters cannot see -- through `.data`, or to inference
+        tensors inside torch.inference_mode() -- need `rebuild=True`: it drops the descriptor, the index lists and
+        the packed words of an unpacked checkpoint and builds them again from the tensors.  Graphs captured before
+        a rebuild point to the dropped buffers: capture them again.
+
         drop_packed=True makes the module DECODE-ONLY: once the index lists exist the packed `indices` are freed
         (4.2 instead of 7.2 bytes per index resident).  Calls with more than one token, `dequant()` and saving the
         state_dict are no longer possible; reloading a checkpoint restores them."""
+        if rebuild:
+            if getattr(self, "_drop_packed", False) and self.indices.numel() == 0:
+                raise RuntimeError("prepare(rebuild=True): this VQuantLinear is decode-only (prepare(drop_packed="
+                                   "True)); its index lists cannot be rebuilt without the packed index words, which "
+                                   "were freed; reload the checkpoint")
+            self._desc_cache, self._desc_key, self._packed = [], None, None
         dtype = dtype or self.centroids.weight.dtype
         x = torch.zeros(1, self.in_features, dtype=dtype, device=self.centroids.weight.device)
         if drop_packed:

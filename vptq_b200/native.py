@@ -33,6 +33,9 @@ EXPORTS = (
     "vptq_b200_lists_build_host", "vptq_b200_quant_gemv_multi_ws", "vptq_b200_tp_untag", "vptq_b200_lists_deal_host",
 )
 
+# CUDA-graph helpers (include/vptq_b200_graph.h), exported from the same library
+GRAPH_EXPORTS = ("vptq_b200_stream_capture_id",)
+
 # training entry points (include/vptq_b200_grad.h), exported from the same library
 GRAD_EXPORTS = ("vptq_b200_grad_version", "vptq_b200_grad_workspace_bytes", "vptq_b200_quant_gemm_wgrad",
                 "vptq_b200_dequant_backward")
@@ -133,6 +136,11 @@ def lib() -> ctypes.CDLL:
         L.vptq_b200_tp_untag.restype = ctypes.c_int
         L.vptq_b200_debug_phase_stamps.argtypes = [vp]
         L.vptq_b200_debug_phase_stamps.restype = None
+        for f in GRAPH_EXPORTS:
+            if not hasattr(L, f):
+                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_graph.h): rebuild it")
+        L.vptq_b200_stream_capture_id.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64)]
+        L.vptq_b200_stream_capture_id.restype = ctypes.c_int
         for f in ("vptq_b200_quant_gemv", "vptq_b200_quant_gemm", "vptq_b200_dequant", "vptq_b200_quant_gemv_v2",
                   "vptq_b200_linear_host"):
             getattr(L, f).restype = ctypes.c_int
@@ -252,8 +260,11 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
     d.bias = _ptr(bias)
     d._keep = ()
     if derive and perm is not None and weight_scale is not None and weight_bias is not None:
-        pidx = perm.view(torch.uint16).to(torch.int64) if perm.dtype in (torch.int16, torch.uint16) else perm.long()
-        ws_q, wb_q = weight_scale[pidx].contiguous(), weight_bias[pidx].contiguous()
+        # ordinary tensors even when built inside torch.inference_mode(): an optimizer step outside it refreshes them
+        # in place (VQuantLinear._refresh_in_place)
+        with torch.inference_mode(False), torch.no_grad():
+            pidx = perm.view(torch.uint16).to(torch.int64) if perm.dtype in (torch.int16, torch.uint16) else perm.long()
+            ws_q, wb_q = weight_scale[pidx].contiguous(), weight_bias[pidx].contiguous()
         d.weight_scale_q, d.weight_bias_q = ws_q.data_ptr(), wb_q.data_ptr()
         d._keep = (ws_q, wb_q)
     if lists is None:
@@ -276,24 +287,70 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
     return d
 
 
-# one zero-initialised workspace per (device, stream): kernels leave it zeroed (include/vptq_b200.h)
-_workspaces: dict = {}
+# Zero-initialised workspaces: kernels leave them zeroed (include/vptq_b200.h).  A CUDA graph keeps the addresses
+# it was captured with, so no buffer a graph may use is freed before release_workspaces() (DESIGN.md section 1).
+_workspaces: dict = {}   # (device, stream) -> the stream's current buffer, zeroed eagerly
+_retired: list = []      # buffers replaced by bigger ones: graphs captured earlier still use them
+_captured: dict = {}     # (device, stream, capture id) -> buffer allocated inside that capture, private to it
+
+
+def _grown(old: Optional[torch.Tensor], nbytes: int) -> int:
+    # at least doubling: everything retired stays below the size of the largest buffer
+    return max(int(nbytes), 1 << 20, 2 * old.numel() if old is not None else 0)
+
+
+def pick_workspace(key, nbytes: int, capture_id: int, alloc, current: dict, retired: list, captured: dict):
+    """The bookkeeping of workspace(), free of CUDA so that it can be tested with fake buffers.
+
+    key: (device, stream); capture_id: the stream's capture id, 0 when it is not capturing; alloc(n): a new
+    zero-initialised buffer of n bytes (inside a capture its fill is recorded into the graph, so it runs only when
+    that graph replays).  An eagerly zeroed buffer that is big enough serves everyone, captures included.  Otherwise
+    a call outside capture replaces it, and a call inside a capture gets a buffer of that capture's own, which no
+    eager call or other capture ever sees.  A replaced buffer is retired, never dropped."""
+    ws = current.get(key)
+    if ws is not None and ws.numel() >= nbytes:
+        return ws
+    if not capture_id:
+        if ws is not None:
+            retired.append(ws)
+        ws = current[key] = alloc(_grown(ws, nbytes))
+        return ws
+    ckey = key + (capture_id,)
+    pv = captured.get(ckey)
+    if pv is not None and pv.numel() >= nbytes:
+        return pv
+    if pv is not None:
+        retired.append(pv)
+    pv = captured[ckey] = alloc(_grown(pv, nbytes))
+    return pv
+
+
+def capture_id(stream: int) -> int:
+    """The id of the CUDA-graph capture running on `stream` (a cudaStream_t handle), 0 when it is not capturing."""
+    cid = ctypes.c_uint64(0)
+    rc = lib().vptq_b200_stream_capture_id(stream, ctypes.byref(cid))
+    if rc < 0:
+        check(rc, "vptq_b200_stream_capture_id")
+    return int(cid.value)
 
 
 def workspace(device: torch.device, nbytes: int) -> torch.Tensor:
-    key = (device.index if device.index is not None else torch.cuda.current_device(),
-           torch.cuda.current_stream(device).cuda_stream)
+    stream = torch.cuda.current_stream(device).cuda_stream
+    key = (device.index if device.index is not None else torch.cuda.current_device(), stream)
     ws = _workspaces.get(key)
-    if ws is None or ws.numel() < nbytes:
-        ws = torch.zeros(max(int(nbytes), 1 << 20), dtype=torch.uint8, device=device)
-        _workspaces[key] = ws
-    return ws
+    if ws is not None and ws.numel() >= nbytes:
+        return ws
+    return pick_workspace(key, nbytes, capture_id(stream),
+                          lambda n: torch.zeros(n, dtype=torch.uint8, device=device), _workspaces, _retired, _captured)
 
 
 def release_workspaces() -> None:
-    """Drop the cached per-stream workspaces (they only grow: a weight-gradient call can leave hundreds of MB).  The
-    next call allocates a fresh zeroed one.  Not while a captured CUDA graph still uses the old ones."""
+    """Drop every cached workspace: the streams' current ones, the retired ones and those private to a capture (they
+    only grow: a weight-gradient call can leave hundreds of MB).  The next call allocates a fresh zeroed one.  Not
+    while a captured CUDA graph still lives: it may use any of them."""
     _workspaces.clear()
+    _retired.clear()
+    _captured.clear()
 
 
 def workspace_bytes(desc: LinearDesc, tokens: int, op: int) -> int:
