@@ -350,6 +350,7 @@ VPTQ_B200_API int vptq_b200_linear_host(const vptq_linear_desc* desc, const void
                           size_t workspace_bytes, uint32_t flags, void* stream);
 
 /* Workspace helpers for hosts that capture CUDA graphs: include/vptq_b200_graph.h. */
+/* Batched decode (2..8 tokens) from the index lists: include/vptq_b200_batch.h. */
 
 #ifdef __cplusplus
 }

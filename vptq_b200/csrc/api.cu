@@ -491,6 +491,47 @@ int vptq_b200_linear_host(const vptq_linear_desc* desc, const void* x_host, void
   return 0;
 }
 
+// ---- batched decode (include/vptq_b200_batch.h) ----
+int vptq_b200_batch_version(void) { return VPTQ_B200_BATCH_VERSION; }
+
+int vptq_b200_quant_gemv_batch_max_tokens(int32_t n, const vptq_linear_desc* const* descs) {
+  if (!descs || n < 1 || n > VPTQ_MAX_FUSED) {
+    set_error("quant_gemv_batch_max_tokens: NULL descs or n %d outside 1..%d", n, VPTQ_MAX_FUSED);
+    return 0;
+  }
+  for (int l = 0; l < n; ++l)
+    if (validate(descs[l], false)) return 0;
+  return gemv_lists_batch_max_tokens(n, descs);
+}
+
+int vptq_b200_quant_gemv_batch(int32_t n, const vptq_linear_desc* const* descs, const void* x, int64_t x_stride,
+                               void* const* ys, const int64_t* y_strides, int32_t tokens, void* workspace,
+                               size_t workspace_bytes, uint32_t flags, void* stream) {
+  if (!descs || !x || !ys || !y_strides || n < 1 || n > VPTQ_MAX_FUSED) {
+    set_error("quant_gemv_batch: NULL argument or n %d outside 1..%d", n, VPTQ_MAX_FUSED);
+    return VPTQ_ERR_INVALID;
+  }
+  if (flags & ~VPTQ_FLAG_PDL) {
+    set_error("quant_gemv_batch: unknown flags 0x%x", flags);
+    return VPTQ_ERR_INVALID;
+  }
+  for (int l = 0; l < n; ++l) {
+    if (int rc = validate(descs[l], l == 0)) return rc;
+    if (!ys[l] || y_strides[l] < descs[l]->out_features || x_stride < descs[l]->in_features) {
+      set_error("quant_gemv_batch: bad y / stride for layer %d", l);
+      return VPTQ_ERR_INVALID;
+    }
+  }
+  const int max_tokens = gemv_lists_batch_max_tokens(n, descs);
+  if (max_tokens == 0) return VPTQ_ERR_UNSUPPORTED;  // (message set)
+  if (tokens < 1 || tokens > max_tokens) {
+    set_error("quant_gemv_batch: %d tokens; these layers take 1..%d", tokens, max_tokens);
+    return VPTQ_ERR_UNSUPPORTED;
+  }
+  return gemv_lists_batch_launch(n, descs, x, x_stride, ys, y_strides, tokens, flags, static_cast<cudaStream_t>(stream),
+                                 workspace, workspace_bytes);
+}
+
 int vptq_b200_stream_capture_id(void* stream, uint64_t* id) {
   if (!id) {
     set_error("stream_capture_id: NULL id");

@@ -8,6 +8,7 @@
 #include "../../include/vptq_b200.h"
 #include "../../include/vptq_b200_grad.h"
 #include "../../include/vptq_b200_graph.h"
+#include "../../include/vptq_b200_batch.h"
 
 namespace vptq_b200 {
 
@@ -105,6 +106,13 @@ int gemv_lists_launch(int n, const vptq_linear_desc* const* descs, const void* x
 size_t gemv_lists_workspace_bytes(const vptq_linear_desc& d);  // 0 when the layer is not eligible
 // tagged-word activation buffer of a VPTQ_TP_TAGGED launch -> plain 16-bit values (waits for the tags)
 int tp_untag_launch(const void* tagged, void* y, int n, const vptq_tp_exchange& tp, cudaStream_t stream);
+
+// Batched variant (gemv_lists_batch.cu, C interface include/vptq_b200_batch.h): 1..8 tokens of layers carrying
+// the same lists, one combo per CTA, every token's sums independent of the others in the launch.
+int gemv_lists_batch_max_tokens(int n, const vptq_linear_desc* const* descs);  // 0: not eligible (error set)
+int gemv_lists_batch_launch(int n, const vptq_linear_desc* const* descs, const void* x, int64_t x_stride,
+                            void* const* ys, const int64_t* y_strides, int tokens, uint32_t flags, cudaStream_t stream,
+                            void* workspace, size_t workspace_bytes);
 
 // -------------------------------------------------------------------------------------------
 // dequant

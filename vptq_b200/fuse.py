@@ -16,6 +16,9 @@ the same tensor (same storage, same version) and only return theirs.  Anything e
 a member called alone, an activation that changed in between -- takes the member's own `forward`, so results
 are those of the unfused model in every case.  `fuse` also builds every layer's descriptor and load-time
 index lists (`VQuantLinear.prepare`), so nothing is allocated or re-bucketed inside the first forward.
+
+After `set_batched_decode(model)` a group whose members all opted in also launches 2..8-token activations as one
+batched list-kernel launch (include/vptq_b200_batch.h), with the same results as its members' own forwards.
 """
 from __future__ import annotations
 
@@ -27,7 +30,7 @@ import torch.nn as nn
 from . import native
 from .layers import VQuantLinear
 
-__all__ = ["fuse", "unfuse", "set_quant_grad", "FusedGroup", "FusedMember", "DEFAULT_GROUPS"]
+__all__ = ["fuse", "unfuse", "set_quant_grad", "set_batched_decode", "FusedGroup", "FusedMember", "DEFAULT_GROUPS"]
 
 DEFAULT_GROUPS: Tuple[Tuple[str, ...], ...] = (("q_proj", "k_proj", "v_proj"), ("gate_proj", "up_proj"))
 
@@ -68,7 +71,11 @@ class FusedGroup:
             return None           # the member's own forward records the autograd graph (same values)
         x2 = x.reshape(-1, x.shape[-1])
         tokens = x2.shape[0]
-        if not x.is_cuda or tokens < 1 or tokens > 2 or x2.stride(-1) != 1 or (tokens > 1 and x2.stride(0) < x2.shape[1]):
+        if not x.is_cuda or tokens < 1 or x2.stride(-1) != 1 or (tokens > 1 and x2.stride(0) < x2.shape[1]):
+            return None
+        # 2..8 tokens: the batched list kernel when every member opted in (set_batched_decode) and it takes them
+        batched = tokens >= 2 and all(getattr(l, "_batched_decode", False) for l in self.layers)
+        if tokens > 2 and not batched:
             return None
         key = activation_key(x)
         if key == self._key and self._out is not None and not (self._served >> index) & 1:
@@ -77,13 +84,18 @@ class FusedGroup:
                 self._key = None
             return self._out
         descs = self._descs(x)
-        fkey = tuple(id(d) for d in descs) + (tokens,)
+        if batched and (x2.data_ptr() % 16 or tokens > native.batch_max_tokens(descs)):
+            if tokens > 2:
+                return None       # each member routes its own call (its own batched launch where it is eligible)
+            batched = False
+        fkey = tuple(id(d) for d in descs) + (tokens, batched)
         if self._fused is None or fkey != self._fused_key:
             self._out = torch.empty(tokens, sum(self.widths), dtype=x.dtype, device=x.device)
             offs = [0]
             for w in self.widths:
                 offs.append(offs[-1] + w)
-            self._fused = native.FusedGemv(descs, [self._out[:, a:b] for a, b in zip(offs[:-1], offs[1:])])
+            fused = native.FusedGemvBatch if batched else native.FusedGemv
+            self._fused = fused(descs, [self._out[:, a:b] for a, b in zip(offs[:-1], offs[1:])])
             self._fused_key = fkey
         self._fused(x2, self.flags)
         self._key, self._served = key, 1 << index
@@ -187,6 +199,16 @@ def set_quant_grad(model: nn.Module, enabled: bool = True) -> int:
             l._check_quant_grad_possible()
     for l in layers:
         l.set_quant_grad(enabled)
+    return len(layers)
+
+
+def set_batched_decode(model: nn.Module, enabled: bool = True) -> int:
+    """`VQuantLinear.set_batched_decode(enabled)` on every VQuantLinear of `model`, fused members included.  Returns
+    how many layers it reached."""
+    layers = [mod.layer if isinstance(mod, FusedMember) else mod for mod in model.modules()]
+    layers = [l for l in layers if isinstance(l, VQuantLinear)]
+    for l in layers:
+        l.set_batched_decode(enabled)
     return len(layers)
 
 

@@ -162,6 +162,7 @@ class VQuantLinear(nn.Module):
         self._desc_key = None
         self._packed = None              # lazily packed indices for unpacked checkpoints
         self._quant_grad = False         # set_quant_grad
+        self._batched_decode = False     # set_batched_decode
 
     # ------------------------------------------------------------------------------------------
     def _tensors(self):
@@ -220,6 +221,16 @@ class VQuantLinear(nn.Module):
         if enabled:
             self._check_quant_grad_possible()
         self._quant_grad = bool(enabled)
+        return self
+
+    def set_batched_decode(self, enabled: bool = True) -> "VQuantLinear":
+        """Opt in to the batched list kernel for 2..8-token calls (several sequences, beams, speculative
+        verification): it reads the index lists once for all tokens instead of dequantising the whole weight
+        (include/vptq_b200_batch.h).  Calls it does not take (1 token, more tokens than it offers, layers without
+        index lists) are routed as without the opt-in.  Its results may differ from the default routes in the low-order
+        bits; each token's outputs do not depend on the other tokens of the call.  A decode-only module
+        (`prepare(drop_packed=True)`) with the opt-in serves 2..8 tokens."""
+        self._batched_decode = bool(enabled)
         return self
 
     def _check_quant_grad_possible(self) -> None:
@@ -325,7 +336,8 @@ class VQuantLinear(nn.Module):
             outlier_size=self.outlier_size, in_features=self.in_features, out_features=self.out_features,
             padding=self.padding, outlier_padding=self.outlier_padding,
             vector_quant_dim=self.vector_quant_dim, _desc_cache=self._desc_cache,
-            _drop_packed=getattr(self, "_drop_request", False), _quant_grad=getattr(self, "_quant_grad", False))
+            _drop_packed=getattr(self, "_drop_request", False), _quant_grad=getattr(self, "_quant_grad", False),
+            _batched_decode=getattr(self, "_batched_decode", False))
 
     def dequant(self) -> torch.Tensor:
         """Dense [out_features, in_features] weight through the CUDA dequant kernel."""

@@ -43,6 +43,10 @@ GRAD_VERSION = 1
 GRAD_OP_WGRAD, GRAD_OP_DEQUANT_BACKWARD, GRAD_OP_WGRAD_GENERIC = 0, 1, 2
 GRAD_FLAG_GENERIC = 1
 
+# batched decode from the index lists (include/vptq_b200_batch.h), exported from the same library
+BATCH_EXPORTS = ("vptq_b200_batch_version", "vptq_b200_quant_gemv_batch_max_tokens", "vptq_b200_quant_gemv_batch")
+BATCH_VERSION = 1
+
 MAX_FUSED, MAX_RANKS = 4, 8
 
 
@@ -159,6 +163,17 @@ def lib() -> ctypes.CDLL:
         L.vptq_b200_dequant_backward.restype = ctypes.c_int
         if L.vptq_b200_grad_version() != GRAD_VERSION:
             raise RuntimeError(f"libvptq_b200.so grad interface {L.vptq_b200_grad_version()} != expected {GRAD_VERSION}")
+        for f in BATCH_EXPORTS:
+            if not hasattr(L, f):
+                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_batch.h): rebuild it")
+        L.vptq_b200_batch_version.restype = ctypes.c_int
+        L.vptq_b200_quant_gemv_batch_max_tokens.argtypes = [i32, ctypes.POINTER(dp)]
+        L.vptq_b200_quant_gemv_batch_max_tokens.restype = ctypes.c_int
+        L.vptq_b200_quant_gemv_batch.argtypes = [i32, ctypes.POINTER(dp), vp, i64, ctypes.POINTER(vp), ctypes.POINTER(i64),
+                                                 i32, vp, sz, u32, vp]
+        L.vptq_b200_quant_gemv_batch.restype = ctypes.c_int
+        if L.vptq_b200_batch_version() != BATCH_VERSION:
+            raise RuntimeError(f"libvptq_b200.so batch interface {L.vptq_b200_batch_version()} != expected {BATCH_VERSION}")
         _lib = L
     return _lib
 
@@ -436,6 +451,58 @@ class FusedGemv:
             self.separate = True              # same kernels, one launch per layer (identical results)
         for d, y in zip(self.descs, self.ys):
             quant_gemv(d, x2d, y, flags)
+
+
+def _desc_array(descs):
+    return (ctypes.POINTER(LinearDesc) * len(descs))(*[ctypes.pointer(d) for d in descs])
+
+
+def batch_max_tokens(descs) -> int:
+    """vptq_b200_quant_gemv_batch_max_tokens: the largest token count the batched list route takes for these layers
+    (one descriptor or a list of 1..MAX_FUSED reading the same x) on the current device, 0 when they are not eligible.
+    Cached on the first descriptor (the answer depends on the shapes and the device only)."""
+    descs = [descs] if isinstance(descs, LinearDesc) else list(descs)
+    if not descs or not all(d.lists_stream for d in descs):
+        return 0
+    idx = torch.cuda.current_device()
+    cache = descs[0].__dict__.setdefault("_batch_max", {})
+    key = (idx,) + tuple(id(d) for d in descs)
+    v = cache.get(key)
+    if v is None:
+        v = cache[key] = int(lib().vptq_b200_quant_gemv_batch_max_tokens(len(descs), _desc_array(descs)))
+    return v
+
+
+def quant_gemv_batch(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, flags: int = 0) -> None:
+    """y2d [tokens, O] = x2d [tokens, I] @ W^T + bias by the batched list kernel (vptq_b200_quant_gemv_batch),
+    1 <= tokens <= batch_max_tokens(desc)."""
+    FusedGemvBatch([desc], [y2d])(x2d, flags)
+
+
+class FusedGemvBatch:
+    """Prepared argument arrays for vptq_b200_quant_gemv_batch (1..MAX_FUSED layers sharing one input, 1..8 tokens).
+    No fall-back: a refusal raises."""
+
+    def __init__(self, descs, ys):
+        n = len(descs)
+        if not 1 <= n <= MAX_FUSED or len(ys) != n:
+            raise RuntimeError(f"FusedGemvBatch takes 1..{MAX_FUSED} layers with one output each")
+        self.n, self.descs, self.ys = n, list(descs), list(ys)
+        self.desc_arr = _desc_array(self.descs)
+        self.y_arr = (ctypes.c_void_p * n)(*[y.data_ptr() for y in ys])
+        self.stride_arr = (ctypes.c_int64 * n)(*[row_pitch(y) for y in ys])
+        self.ws_bytes = None
+
+    def __call__(self, x2d: torch.Tensor, flags: int = 0) -> None:
+        dev = x2d.device
+        with _on_device(dev):
+            if self.ws_bytes is None:
+                self.ws_bytes = sum(_ws_bytes_cached(d, 1, OP_GEMV) for d in self.descs)
+            ws = workspace(dev, self.ws_bytes)
+            rc = lib().vptq_b200_quant_gemv_batch(self.n, self.desc_arr, x2d.data_ptr(), row_pitch(x2d), self.y_arr,
+                                                  self.stride_arr, x2d.shape[0], ws.data_ptr(), ws.numel(), flags,
+                                                  _stream(dev))
+        check(rc, "vptq_b200_quant_gemv_batch")
 
 
 class FusedGemvTP:

@@ -7,7 +7,8 @@ Function names, argument order and argument meaning are the reference's
 * every op runs hand-written sm_90a CUDA through the C ABI (vptq_b200.native); there is no
   torch implementation to fall back to -- CPU tensors raise;
 * routing: fewer than 3 tokens -> fused GEMV (the reference's rule, :213); otherwise the fused
-  dequant->wgmma GEMM instead of `dequant` + `F.linear` (:231-275);
+  dequant->wgmma GEMM instead of `dequant` + `F.linear` (:231-275).  Opt-in (`_batched_decode`,
+  VQuantLinear.set_batched_decode): 2..8 tokens of a layer with index lists -> the batched list kernel;
 * `argsort(perm)` is not recomputed on every call (the reference does, :208-211).
 """
 from __future__ import annotations
@@ -173,11 +174,15 @@ def quant_gemm(
     _desc_cache: Optional[list] = None,
     _drop_packed: bool = False,
     _quant_grad: bool = False,
+    _batched_decode: bool = False,
 ) -> torch.Tensor:
     """y = x @ W^T + bias for one VPTQ layer (reference: vptq/ops/quant_gemm.py:161-275).
 
     `_quant_grad` (VQuantLinear.set_quant_grad): under grad mode the codebooks, weight_scale and weight_bias that
-    require grad get gradients too, also when x does not require grad (vptq_b200_quant_gemm_wgrad)."""
+    require grad get gradients too, also when x does not require grad (vptq_b200_quant_gemm_wgrad).
+
+    `_batched_decode` (VQuantLinear.set_batched_decode): 2..batch_max_tokens tokens of a layer that carries index
+    lists run the batched list kernel (include/vptq_b200_batch.h); every other call is routed as without it."""
     if vector_quant_dim == "in":
         raise ValueError("Not implemented yet.")
     if not is_indice_packed:
@@ -218,21 +223,25 @@ def quant_gemm(
             if not quant:
                 layer = (indices, centroids, residual_centroids, outlier_indices, outlier_centroids, perm,
                          weight_scale, weight_bias)
-                y = _QuantLinearFn.apply(x2d, bias, keep, out_features, *[t for t in layer if t is not None])
+                y = _QuantLinearFn.apply(x2d, bias, keep, out_features, _batched_decode,
+                                         *[t for t in layer if t is not None])
             else:
                 others = [t for t in (indices, outlier_indices, perm) if t is not None]
-                y = _QuantLinearWgradFn.apply(x2d, bias, keep, out_features, tuple(n for n, _ in slots),
-                                              *[t for _, t in slots], *others)
+                y = _QuantLinearWgradFn.apply(x2d, bias, keep, out_features, _batched_decode,
+                                              tuple(n for n, _ in slots), *[t for _, t in slots], *others)
             return y.reshape(*x.shape[:-1], out_features)
-    return _forward(desc, x2d, out_features).reshape(*x.shape[:-1], out_features)
+    return _forward(desc, x2d, out_features, _batched_decode).reshape(*x.shape[:-1], out_features)
 
 
-def _forward(desc, x2d: torch.Tensor, out_features: int) -> torch.Tensor:
+def _forward(desc, x2d: torch.Tensor, out_features: int, batched: bool = False) -> torch.Tensor:
     tokens = x2d.shape[0]
     y = torch.empty(tokens, out_features, dtype=x2d.dtype, device=x2d.device)
     if tokens == 0:
         return y
-    if tokens < 3:
+    if batched and tokens >= 2 and desc.lists_stream and x2d.data_ptr() % 16 == 0 and \
+            tokens <= native.batch_max_tokens(desc):
+        native.quant_gemv_batch(desc, x2d, y)
+    elif tokens < 3:
         native.quant_gemv(desc, x2d, y)
     else:
         native.quant_gemm(desc, x2d, y)
@@ -249,17 +258,17 @@ class _QuantLinearFn(torch.autograd.Function):
     in-place update between forward and backward fails autograd's version check instead of using new weights."""
 
     @staticmethod
-    def forward(ctx, x2d, bias, keep, out_features, *layer):
+    def forward(ctx, x2d, bias, keep, out_features, batched, *layer):
         ctx.keep = keep
         ctx.save_for_backward(*layer)
-        return _forward(keep[0], x2d, out_features)
+        return _forward(keep[0], x2d, out_features, batched)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, dy):
         ctx.saved_tensors            # version check of the layer tensors
         dx, dbias = _input_grads(ctx, ctx.keep[0], dy)
-        return (dx, dbias, None, None) + (None,) * len(ctx.saved_tensors)
+        return (dx, dbias, None, None, None) + (None,) * len(ctx.saved_tensors)
 
 
 def _input_grads(ctx, desc, dy):
@@ -287,10 +296,10 @@ class _QuantLinearWgradFn(torch.autograd.Function):
     autograd's version check)."""
 
     @staticmethod
-    def forward(ctx, x2d, bias, keep, out_features, names, *layer):
+    def forward(ctx, x2d, bias, keep, out_features, batched, names, *layer):
         ctx.keep, ctx.names = keep, names
         ctx.save_for_backward(x2d, *layer)
-        return _forward(keep[0], x2d, out_features)
+        return _forward(keep[0], x2d, out_features, batched)
 
     @staticmethod
     @once_differentiable
@@ -299,14 +308,14 @@ class _QuantLinearWgradFn(torch.autograd.Function):
         x2d, quant = saved[0], saved[1:1 + len(ctx.names)]
         desc = ctx.keep[0]
         dx, dbias = _input_grads(ctx, desc, dy)
-        want = _quant_grads(ctx, 5, ctx.names, quant)
+        want = _quant_grads(ctx, 6, ctx.names, quant)
         if want:
             if dy.shape[0]:
                 native.quant_gemm_wgrad(desc, x2d, dy, want)
             else:
                 for t in want.values():
                     t.zero_()
-        return (dx, dbias, None, None, None) + tuple(want.get(n) for n in ctx.names) + \
+        return (dx, dbias, None, None, None, None) + tuple(want.get(n) for n in ctx.names) + \
             (None,) * (len(saved) - 1 - len(quant))
 
 
