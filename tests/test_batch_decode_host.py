@@ -88,10 +88,10 @@ def kernel_split(Ro, Q, firsts, tokens):
     return ctas
 
 
-def carve(TCW, max_nun, max_kr, ntok, limit=SMEM_OPTIN):
+def carve(TCW, max_nun, max_kr, ntok, limit=SMEM_OPTIN, stages_tried=(3, 2)):
     """shared-memory bytes of instance ntok (batch_carve), 0: nothing fits"""
     al = lambda v: (v + 127) // 128 * 128
-    for stages in (3, 2):
+    for stages in stages_tried:
         off = al((1 + WARPS * stages) * 8) + al((max_nun + 1) * 4) + al((WARPS + 1) * MAX_TOK * 4 + 16)
         off += al(WARPS * 2 * ntok * 32 + WARPS * 2 * 4) + al((max_nun // RB + 2) * 4) + 65536
         off += al(max_kr * 16 * 8) + al(TCW * ntok * 2) + WARPS * stages * STAGE_STEPS * 128
@@ -162,6 +162,64 @@ def test_eligibility_limits():
     assert partition([512, 512], 132) is None                 # n * Q > SM count
     assert partition([512], 132) == [1]
     assert partition([4096 // 8, 128, 128], 16) == [5, 2, 1]  # 8B q/k/v: 128 of 132 SMs
+
+
+def _plan(I, outs, K=65536, Kr=256):
+    """(Q, k, the carve of NTOK = 2, 4, 8, the same with 3 ring stages only) of a fused set, as the kernel plans it"""
+    from vptq_b200 import lists
+    ns, nt, tcw = lists.geometry(I, K)
+    Q, Ro = ns * nt, [(o + 7) // 8 for o in outs]
+    k = partition(Ro, Q)
+    if k is None:
+        return Q, None, None, None
+    mn = max((r + kl - 1) // kl for r, kl in zip(Ro, k))
+    return (Q, k, [carve(tcw, mn, Kr, n) for n in (2, 4, 8)],
+            [carve(tcw, mn, Kr, n, stages_tried=(3,)) for n in (2, 4, 8)])
+
+
+# the cut-off shapes of tests/test_gpu_batch_envelope.py, each on its intended side
+def test_cutoff_ring_stages():
+    """I = 12288, two 20480-output layers: NTOK = 8 needs the 2-stage ring, NTOK = 2 and 4 keep 3 stages; the 70B
+    gate+up pair keeps 3 stages at NTOK = 8 (2432 bytes to spare)"""
+    Q, k, both, three = _plan(12288, [20480, 20480])
+    assert Q == 48 and k == [1, 1]
+    assert three[0] == both[0] > 0 and three[1] == both[1] > 0
+    assert three[2] == 0 and both[2] == 216704
+    Q, k, both, three = _plan(8192, [28672, 28672])
+    assert Q == 32 and k == [2, 2] and three == both and SMEM_OPTIN - both[2] == 2432
+
+
+def test_cutoff_last_layout_that_fits():
+    """I = 20480 (Q = 80), Kr = 256: out = 51192 fits with 0 bytes to spare, out = 51200 does not fit"""
+    Q, k, both, _ = _plan(20480, [51192])
+    assert Q == 80 and k == [1] and both[2] == SMEM_OPTIN
+    Q, k, both, _ = _plan(20480, [51200])
+    assert both[2] == 0 and both[0] > 0 and both[1] > 0      # batch_max_tokens asks for NTOK = 8: 0
+
+
+def test_cutoff_workspace_rows():
+    """sum Ro x 8 = 65536 accepted (one layer, and 4 fused layers), 65544 refused"""
+    assert _plan(4096, [65536])[1] == [8]
+    assert _plan(4096, [16384] * 4)[1] == [2, 2, 2, 2]
+    assert _plan(4096, [65544])[1] is None
+    assert partition([65536 // 8], 16) is not None and partition([65544 // 8], 16) is None
+
+
+def test_cutoff_partition_regimes():
+    """n = B; n > B (three layers at I = 12288); B = 1 (Q = 128); k = Ro; Ro = 1; ragged multi-tile widths"""
+    assert _plan(14336, [4096, 4096])[:2] == (64, [1, 1])
+    assert SM_COUNT // 48 == 2 and _plan(12288, [4096, 1024, 1024])[1] is None
+    assert all(_plan(12288, [o])[1] is not None for o in (4096, 1024))
+    assert _plan(32768, [4096])[:2] == (128, [1])
+    assert _plan(1024, [264], K=8192)[:2] == (2, [33])
+    assert _plan(1024, [8])[:2] == (16, [1])
+    from vptq_b200 import lists
+    assert lists.geometry(4100, 65536) == (16, 2, 2056) and 4100 - 2056 == 2044
+    assert lists.geometry(9004, 65536) == (16, 3, 3008) and 9004 % 8 != 0
+    # a valid codebook is a power of two (NS in {2, 4, 8, 16}) and NT <= 16: NS x NT never equals 132
+    assert not [(ns, nt) for ns in (2, 4, 8, 16) for nt in range(1, 17) if ns * nt == SM_COUNT]
+    for I, outs in FUSED_SETS.values():                       # every full-size set also fits at NTOK = 8
+        assert _plan(I, outs)[2][2] > 0
 
 
 # ---------------------------------------------------------------- python routing with native stubbed

@@ -14,8 +14,8 @@ from _util import TOL
 
 pytestmark = pytest.mark.gpu
 
-BATCH = "gemv_lists_batch_kernel"
-ZERO_HEAD = 65536 * 4 + 65536 * 64   # kZeroRegionBytes: the workspace head kernels leave zeroed
+from _batch import BATCH, ZERO_HEAD, assert_close, batch as _batch, desc_of as _desc, head_zero as _head_zero, q_of
+from _batch import kernel_star as _kernel_star
 
 CASES = {
     "4096x4096_r256": dict(in_features=4096, out_features=4096, num_centroids=65536, num_res_centroids=256),
@@ -41,28 +41,8 @@ def _layer(name):
     return _layers[name]
 
 
-def _desc(L):
-    from _gpu import tdtype, to_t
-    from vptq_b200 import native
-    t = dict(indices=to_t(L.indices, L, "i32"), centroids=to_t(L.centroids, L),
-             res_centroids=to_t(L.res_centroids, L) if L.res_bits else None,
-             perm=to_t(L.perm, L, "u16") if L.perm is not None else None,
-             weight_scale=to_t(L.weight_scale, L) if L.weight_scale is not None else None,
-             weight_bias=to_t(L.weight_bias, L) if L.weight_bias is not None else None,
-             bias=to_t(L.bias, L) if L.bias is not None else None)
-    d = native.make_desc(dtype=tdtype(L), in_features=L.in_features, out_features=L.out_features, vector_len=8,
-                         num_centroids=L.num_centroids, num_res_centroids=L.num_res_centroids, num_codebooks=1,
-                         group_size=L.group_size, outlier_size=0, outlier_vector_len=-1, num_outlier_centroids=-1,
-                         outlier_indices=None, outlier_centroids=None, lists=True, **t)
-    d._tensors = t
-    assert d.lists_stream
-    return d
-
-
 def _q(L):
-    from vptq_b200.lists import geometry
-    ns, nt, _ = geometry(L.in_features, L.num_centroids)
-    return ns * nt
+    return q_of(L.in_features, L.num_centroids)
 
 
 def _x(L, tokens, seed):
@@ -70,52 +50,8 @@ def _x(L, tokens, seed):
     return x_to_t(vo.make_x(tokens, L.in_features, L.dtype, seed=seed), L)
 
 
-def _batch(descs, x, ys=None, flags=0):
-    from vptq_b200 import native
-    single = not isinstance(descs, (list, tuple))
-    descs = [descs] if single else list(descs)
-    if ys is None:
-        ys = [torch.full((x.shape[0], d.out_features), float("nan"), dtype=x.dtype, device=x.device) for d in descs]
-    native.FusedGemvBatch(descs, ys)(x, flags)
-    return ys[0] if single else ys
-
-
-def _kernel_star(L, x):
-    """fp64 evaluation of the kernel's arithmetic: rn16(x * s) . (C + R)^T [C + R rounded to fp16 for fp16 layers]
-    + x . wbias + bias, as element-wise products (inf * 0 = NaN, like the kernel)"""
-    import _extreme as ex
-    P = ex.copy_layer(L)
-    dt = torch.float16 if L.dtype == "fp16" else torch.bfloat16
-    if P.weight_scale is not None:
-        s = torch.from_numpy(vo.to_f32(L.weight_scale, L.dtype)).to(x.device)
-        wb = torch.from_numpy(vo.to_f32(L.weight_bias, L.dtype).astype(np.float64)).to(x.device)
-        P.weight_scale = ex.encode(np.ones(L.in_features), L.dtype)
-        P.weight_bias = ex.encode(np.zeros(L.in_features), L.dtype)
-        xq = (x.float() * s).to(dt).double()
-    else:
-        wb, xq = None, x.double()
-    P.bias = None
-    W = torch.from_numpy(ex.dense64(P)).to(x.device)             # C + R in fp64 (scale 1, bias 0)
-    if L.dtype == "fp16":
-        W = W.half().double()                                    # packed fp16 c + r
-    y = ex.ew_matmul(xq, W, ex.bias64(L, x.device))
-    if wb is not None:
-        y = y + ex.ew_matmul(x.double(), wb[None, :])
-    return y
-
-
 def _assert_close(y, ystar, L, factor=1.0):
-    q = _q(L)
-    for t in range(y.shape[0]):
-        bar = factor * (TOL[L.dtype] * float(ystar[t].abs().max()) + q * 2.0 ** -31)
-        err = float((y[t].double() - ystar[t]).abs().max())
-        assert err <= bar, (t, err, bar)
-
-
-def _head_zero():
-    from vptq_b200 import native
-    for ws in list(native._workspaces.values()) + list(native._captured.values()):
-        assert int(ws[:ZERO_HEAD].count_nonzero()) == 0
+    assert_close(y, ystar, L.dtype, _q(L), factor)
 
 
 # ---------------------------------------------------------------- probes

@@ -26,6 +26,8 @@ from _extreme import (FINITE, NAN, NEG_INF, POS_INF, VALUES, classify, dense64, 
 from _probe import launched_kernels, ran
 from _util import TOL, parity_error
 
+import _batch
+
 pytestmark = pytest.mark.gpu
 
 
@@ -111,7 +113,7 @@ class Ctx:
             main[4096] = ROWS["Cs"]
         self.L = isolate(L, main=main, res={R_ARB: ROWS["Rk"], 0: ROWS["R0"]} if L.res_bits else None)
         self.W = torch.from_numpy(dense64(self.L)).cuda()
-        self.x = torch.from_numpy(vo.to_f32(vo.make_x(3, L.in_features, L.dtype, seed=17), L.dtype)).cuda().to(_dt(L))
+        self.x = torch.from_numpy(vo.to_f32(vo.make_x(8, L.in_features, L.dtype, seed=17), L.dtype)).cuda().to(_dt(L))
         self.dy = torch.from_numpy(vo.to_f32(vo.make_x(3, L.out_features, L.dtype, seed=18), L.dtype)).cuda().to(_dt(L))
         self._d = {}
 
@@ -153,6 +155,10 @@ def run(kind, c, x, descs=None):
         f(x)
         assert not f.separate
         y = torch.cat(ys, dim=1)
+    elif kind == "batch":
+        y = _batch.batch(c.desc(True), x)
+    elif kind == "batch_fused":
+        y = torch.cat(_batch.batch(descs, x), dim=1)
     else:
         raise ValueError(kind)
     return y
@@ -163,6 +169,8 @@ def kernels_ok(kind, names):
     return {
         "lists": ran(names, "gemv_lists_kernel") and not ran(names, "gemv_kernel"),
         "fused": sum(ran([n], "gemv_lists_kernel") for n in names) == 1 and not ran(names, "gemv_kernel"),
+        "batch": sum(ran([n], _batch.BATCH) for n in names) == 1 and not ran(names, "gemv_lists_kernel"),
+        "batch_fused": sum(ran([n], _batch.BATCH) for n in names) == 1 and not ran(names, "gemv_lists_kernel"),
         "generic": ran(names, "gemv_kernel") and not ran(names, "gemv_lists_kernel"),
         "direct": ran(names, "dequant_o8_kernel") and ran(names, "gemm_tn_wgmma") and not ran(names, "prefill_prep_x"),
         "prep": ran(names, "prefill_prep_x") and ran(names, "gemm_tn_wgmma") and not ran(names, "dequant_o8_kernel"),
@@ -197,7 +205,10 @@ ROUTES = {
     "prep_bf16": ("i1000_bf16", "prep", 3),
     "dequant": ("i1004", "dequant", 0),
     "dgrad": ("i1004", "dgrad", 3),
+    **{f"batch{t}_{cfg}": (cfg, "batch", t) for cfg in ("i1004", "i1000_bf16", "i9000", "llama") for t in (2, 5, 8)},
+    "batch_fused": ("i1004", "batch_fused", 5),
 }
+LISTS_LIKE = ("lists", "fused", "batch", "batch_fused")     # kinds that run a list kernel (descriptors with lists)
 
 
 def _sites(route):
@@ -210,7 +221,7 @@ def _sites(route):
     s = ["C_arb", "C0", "Rk", "R0", "scale", "wbias"]
     if kind != "dequant":
         s.insert(0, "x")
-    if kind == "lists":
+    if kind in ("lists", "batch", "batch_fused"):
         s.append("Cs")
     if kw.get("bias") and kind not in ("dequant", "dgrad"):
         s.append("bias")
@@ -268,7 +279,7 @@ def test_injection(route, site, monkeypatch):
         monkeypatch.setenv("VPTQ_B200_GEMM_PREP", "1")
     c = ctx(cfg)
     descs = None
-    if kind == "fused":
+    if kind in ("fused", "batch_fused"):
         descs = [c.desc(True), ctx("fused_1").desc(True), ctx("fused_2").desc(True)]
     x = c.dy if kind == "dgrad" else c.x[:max(tokens, 1)]
     clean = run_checked(kind, c, x, descs)
@@ -280,23 +291,23 @@ def test_injection(route, site, monkeypatch):
         else:
             kw, field = _injection(c, site, v)
             Li = inject(c.L, value=v, **kw)
-            upload(c.desc(kind == "lists" or kind == "fused"), Li, field)
+            upload(c.desc(kind in LISTS_LIKE), Li, field)
             if field != "bias":
                 W = torch.from_numpy(dense64(Li)).cuda()
         try:
             y = run(kind, c, xi, descs)
         finally:
             if field is not None:
-                upload(c.desc(kind == "lists" or kind == "fused"), c.L, field)
+                upload(c.desc(kind in LISTS_LIKE), c.L, field)
         if kind == "dequant":
             ys = W
         elif kind == "dgrad":
             ys = dgrad_star(Li, xi, W)
-        elif kind == "fused":
+        elif kind in ("fused", "batch_fused"):
             ys = torch.cat([y_star(Li, xi, W)] + [y_star(ctx(n).L, xi, ctx(n).W) for n in ("fused_1", "fused_2")], 1)
         else:
             ys = y_star(Li, xi, W)
-        check_classes(y, ys, clean, vname, site, kind in ("lists", "fused"))
+        check_classes(y, ys, clean, vname, site, kind in LISTS_LIKE)
         assert torch.equal(run(kind, c, x, descs), clean), "a clean call after the poisoned one differs"
 
 
@@ -516,3 +527,137 @@ def test_lists_scaling_within_the_documented_floor(dtype, ks):
         assert err <= bound, (k, err, bound)
     if dtype == "bf16":
         assert smallest < 2.0 ** -22            # the sweep reached outputs where only the floor holds
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the batched list kernel (2..8 tokens per launch)
+# ------------------------------------------------------------------------------------------------------------------
+def test_batch_padding_targets_of_every_slice():
+    """padding lanes decode to entry s 4096 of their unit's slice and to residual entry 0: all sixteen such main
+    entries and residual entry 0, confined to rows 1..18 and set to NaN, reach no other output"""
+    L = vo.make_layer(vector_len=8, seed=4243, **CONFIGS["i1004"])
+    rows = {s * 4096: [1 + s] for s in range(16)}
+    L = isolate(L, main=rows, res={0: [17, 18]})
+    P, bad = {}, L
+    for k in rows:
+        for e in range(8):
+            bad = inject(bad, "C", float("nan"), k=k, e=e)
+    for e in range(8):
+        bad = inject(bad, "R", float("nan"), k=0, e=e)
+    d_clean, d_bad = _batch.desc_of(L), _batch.desc_of(bad)
+    hit = torch.zeros(L.out_features, dtype=torch.bool, device="cuda")
+    hit[8:19 * 8] = True
+    x = ctx("i1004").x
+    for tokens in (2, 5, 8):
+        clean = _batch.batch(d_clean, x[:tokens])
+        names = launched_kernels(lambda: P.update(y=_batch.batch(d_bad, x[:tokens])))
+        assert kernels_ok("batch", names), names
+        y = P["y"]
+        assert torch.equal(y[:, ~hit], clean[:, ~hit]), tokens
+        assert bool(torch.isnan(y[:, hit]).all()), tokens
+    _batch.head_zero()
+
+
+@pytest.mark.parametrize("second_unit", [False, True])
+def test_batch_fp16_past_the_fixed_point_range_one_token_of_five(second_unit):
+    """token 2 of 5 hits entries of 60000 with x = 60000: alone, one slice-0 unit of three such terms (1.08e10, past
+    2^33); with `second_unit`, two units (slices 0 and 1) of two terms each (7.2e9 each: inside 2^33, past
+    2^33 / 2^ceil(log2 Q) = 2^32, and their 2^-30 fixed-point sum past 2^63).  +inf or NaN, never -inf or finite;
+    the other four tokens (small x) bit-identical to a batch in which token 2 is small too"""
+    L = _const_layer(60000.0)
+    idx = L.meta["idx"]
+    split = 2 if second_unit else 3
+    idx[0, :, :split] = idx[0, :, :split] % 4096                      # slice 0
+    idx[0, :, split:4] = 4096 + idx[0, :, split:4] % 4096             # slice 1
+    L.indices = vo.pack_index(idx, L.index_bits)
+    c = Plain(L)
+    x = (_sweep_x(5, 1024, "fp16", seed=13) * 2.0 ** -10).half()
+    clean = run_checked("batch", c, x)
+    assert torch.isfinite(clean).all()
+    xb = x.clone()
+    xb[2, :4 if second_unit else 3] = 60000.0
+    assert bool((y_star(L, xb[2:3], c.W) > 1e10).all())
+    y = run_checked("batch", c, xb)
+    assert bool(((y[2] == float("inf")) | torch.isnan(y[2])).all()), y[2]
+    others = [0, 1, 3, 4]
+    assert torch.equal(y[others], clean[others])
+    _batch.head_zero()
+
+
+def test_batch_bf16_outputs_beyond_the_fixed_point_range():
+    """the 2^36 entry of test_bf16_outputs_beyond_the_fixed_point_range in a 5-token batch: NaN or correct at the hit
+    outputs, correct everywhere else"""
+    L = _bf16_layer()
+    L = isolate(L, main={K_ARB: [1, 7]})
+    e = 3
+    L = inject(L, "C", 2.0 ** 36, k=K_ARB, e=e)
+    x = torch.from_numpy(vo.to_f32(vo.make_x(5, 1024, "bf16", seed=3), "bf16")).cuda().to(torch.bfloat16)
+    for r in (1, 7):
+        f = feature_of(L, isolated_column(L, r, K_ARB))
+        x[:, f] = 1.0
+        s = vo.to_f32(L.weight_scale, "bf16")
+        s[f] = 1.0
+        L.weight_scale = encode(s, "bf16")
+    c = Plain(L)
+    ys = y_star(L, x, c.W)
+    hit = torch.zeros(L.out_features, dtype=torch.bool, device="cuda")
+    hit[[8 + e, 56 + e]] = True
+    assert bool((ys[:, hit].abs() >= 2.0 ** 33).all())
+    y = run_checked("batch", c, x).double()
+    rest = float((y[:, ~hit] - ys[:, ~hit]).abs().max() / ys[:, ~hit].abs().max())
+    assert rest <= TOL["bf16"], rest
+    ok = ((y[:, hit] - ys[:, hit]).abs() / ys[:, hit].abs() <= TOL["bf16"]) | torch.isnan(y[:, hit])
+    assert bool(ok.all()), y[:, hit]
+    _batch.head_zero()
+
+
+@pytest.mark.parametrize("dtype,ks", [("fp16", (-8, -6, -4, -2, 0, 3, 6, 8)), ("bf16", (-24, -19, -14, -9, -4, 0, 4, 8))],
+                         ids=["fp16", "bf16"])
+def test_batch_magnitude_spread(dtype, ks):
+    """one 8-token batch whose tokens are scaled by 2^k, k spread over the range: each token within its own bar (the
+    kernel's arithmetic in fp64; twice that against the exact product) and the same bits as that token alone"""
+    c = Plain(_sweep_layer(dtype, 1004))
+    q = _batch.q_of(1004, c.L.num_centroids)
+    x = _sweep_x(8, 1004, dtype, seed=14) * torch.tensor([2.0 ** k for k in ks], device="cuda")[:, None]
+    x = x.to(_dt(c.L))
+    y = run_checked("batch", c, x)
+    kstar, ys = _batch.kernel_star(c.L, x), y_star(c.L, x, c.W)
+    for t in range(8):
+        _batch.assert_close(y[t:t + 1], kstar[t:t + 1], dtype, q)
+        _batch.assert_close(y[t:t + 1], ys[t:t + 1], dtype, q, factor=2.0)
+        assert torch.equal(run("batch", c, x[t:t + 1].clone()), y[t:t + 1]), t
+    _batch.head_zero()
+
+
+def test_batch_graph_replay_poisoned_then_clean():
+    """CUDA graph of the batched route: one capture of a 5-token launch, replayed with clean, poisoned and clean x"""
+    from vptq_b200 import native
+    c = ctx("i1004")
+    d = c.desc(True)
+    xbuf = c.x[:5].clone()
+    y = torch.empty(5, c.L.out_features, dtype=xbuf.dtype, device="cuda")
+    fb = native.FusedGemvBatch([d], [y])
+    assert kernels_ok("batch", launched_kernels(lambda: fb(xbuf)))
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        fb(xbuf, native.FLAG_PDL)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, stream=s):
+            fb(xbuf, native.FLAG_PDL)
+    g.replay()
+    torch.cuda.synchronize()
+    clean = y.clone()
+    for vname, v in VALUES.items():
+        xi = c.x[:5].clone()
+        xi[3, 10] = v
+        xbuf.copy_(xi)
+        y.fill_(0)
+        g.replay()
+        torch.cuda.synchronize()
+        check_classes(y, y_star(c.L, xi, c.W), clean, vname, "x", True)
+        xbuf.copy_(c.x[:5])
+        g.replay()
+        torch.cuda.synchronize()
+        assert torch.equal(y, clean), vname
+    _batch.head_zero()

@@ -62,6 +62,8 @@ KERNELS = {
     "generic": lambda n: ran(n, "gemv_kernel") and not ran(n, "gemv_lists_kernel"),
     "direct": lambda n: ran(n, "dequant_o8_kernel") and ran(n, "gemm_tn_wgmma") and not ran(n, "prefill_prep_x"),
     "prep": lambda n: ran(n, "prefill_prep_x") and ran(n, "gemm_tn_wgmma") and not ran(n, "dequant_o8_kernel"),
+    "batch": lambda n: sum(ran([k], "gemv_lists_batch_kernel") for k in n) == 1 and not ran(n, "gemv_lists_kernel")
+    and not ran(n, "gemv_kernel") and not ran(n, "gemm_tn_wgmma"),
 }
 
 
@@ -696,3 +698,282 @@ def test_c4_prepared_in_inference_mode_then_trained():
                 assert same(l(x300), fresh(x300)), (step, n)
                 assert l._desc_cache[0] is descs[k], (step, n)
     assert losses[-1] < losses[0], losses
+
+
+# ================================================================================================ batched decode
+def batched(L):
+    return make_module(L).set_batched_decode(True)
+
+
+def test_batch_graphs_across_growth_capture_streams_and_a_second_stream():
+    """A1 + A2 + A6 for the batched route: a graph captured on a side stream survives eager workspace growth; a graph
+    captured on torch's capture stream (a workspace private to the capture) replays last-captured first; a batched
+    stream and a single-token list stream run at once"""
+    from vptq_b200 import native
+    L, Lp = layer("lists"), layer("prep")
+    m, mp, m1 = batched(L), make_module(Lp), make_module(L)
+    x5, x8, x1 = xs(L, 5, seed=5), xs(L, 8, seed=8), xs(L, 1, seed=1)
+    assert_route("batch", lambda: m(x5))
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s), torch.no_grad():
+        e5, e8 = m(x5), m(x8)
+        g5 = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g5, stream=s):
+            y5 = m(x5)
+        old = weakref.ref(native._workspaces[ws_key(s)])
+        for t in (300, 8192):
+            x = xs(Lp, t, seed=t)
+            close64(Lp, x, mp(x))
+        assert native._workspaces[ws_key(s)] is not old()
+    assert old() is not None
+    torch.cuda.current_stream().wait_stream(s)
+    with torch.no_grad():
+        g8 = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g8):
+            y8 = m(x8)
+    assert ws_key(torch.cuda.graphs.graph.default_capture_stream) not in native._workspaces
+    with torch.no_grad():
+        for rep in range(3):
+            g8.replay()
+            with torch.cuda.stream(s):
+                g5.replay()
+            assert same(m(x5), e5)
+            torch.cuda.synchronize()
+            assert same(y8, e8) and same(y5, e5), rep
+        serial1 = m1(x1)
+        streams = [torch.cuda.Stream(), torch.cuda.Stream()]
+        for st in streams:
+            st.wait_stream(torch.cuda.current_stream())
+        outs = [[], []]
+        for _ in range(30):
+            with torch.cuda.stream(streams[0]):
+                outs[0].append(m(x8))
+            with torch.cuda.stream(streams[1]):
+                outs[1].append(m1(x1))
+    torch.cuda.synchronize()
+    assert all(same(y, e8) for y in outs[0]) and all(same(y, serial1) for y in outs[1])
+    close64(L, x5, e5)
+    close64(L, x8, e8)
+    heads_at_rest()
+
+
+def test_batch_on_the_shared_workspace():
+    """A5: the batched route interleaved with every other op on one stream's workspace, each result the bits of the
+    op alone"""
+    from vptq_b200 import native
+    ops = _ops()
+    L = layer("lists")
+    mb = batched(L)
+    x5 = xs(L, 5, seed=55)
+    ops["batch"] = lambda: mb(x5)
+    alone = {}
+    for name, fn in ops.items():
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s), torch.no_grad():
+            alone[name] = fn()
+        s.synchronize()
+    close64(L, x5, alone["batch"])
+    names = list(ops) + ["batch"] * 4
+    random.Random(6).shuffle(names)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s), torch.no_grad():
+        for name in names:
+            y = ops[name]()
+            s.synchronize()
+            assert int(native._workspaces[ws_key(s)][:ZERO].count_nonzero()) == 0, name
+            assert same(y, alone[name]), name
+    heads_at_rest()
+
+
+@pytest.mark.parametrize("update", ["mul", "adam"])
+def test_batch_graph_after_in_place_updates(update):
+    """B1: mul_ or an Adam step on every float tensor (weight_scale / weight_bias are read in original order by this
+    kernel), prepare(), then replay: the bits of a fresh module with batched decode on"""
+    L = layer("lists")
+    m = batched(L)
+    m.prepare()
+    x = xs(L, 6, seed=6)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s), torch.no_grad():
+        m(x)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, stream=s):
+            y = m(x)
+    torch.cuda.current_stream().wait_stream(s)
+    params = [m.centroids.weight, m.res_centroids.weight, m.weight_scale, m.weight_bias, m.bias]
+    if update == "mul":
+        with torch.no_grad():
+            for k, p in enumerate(params):
+                p.mul_(1.0 + 0.125 * (k + 1))
+    else:
+        m.set_quant_grad(True)
+        for p in params:
+            p.requires_grad_(True)
+        opt = torch.optim.Adam(params, lr=1e-3, eps=1e-4)
+        m(xs(L, 64, seed=30)).float().square().mean().backward()
+        opt.step()
+        m.set_quant_grad(False)
+    m.prepare()
+    fresh = fresh_of(m, L).set_batched_decode(True)
+    with torch.cuda.stream(s):
+        g.replay()
+    torch.cuda.synchronize()
+    with torch.no_grad():
+        assert_route("batch", lambda: fresh(x))
+        assert same(y, fresh(x))
+        for t in (2, 5, 8):
+            xt = xs(L, t, seed=70 + t)
+            assert same(m(xt), fresh(xt)), t
+    close64(layer_of(m, L), x, y)
+    heads_at_rest()
+
+
+@pytest.mark.parametrize("change", ["copy_indices", "permute_perm", "load_state_dict"])
+def test_batch_eager_after_changes(change):
+    """B2 for the batched route"""
+    L, Lo = layer("lists"), layer("other")
+    m, other = batched(L), make_module(Lo)
+    with torch.no_grad():
+        m(xs(L, 5))
+        if change == "copy_indices":
+            m.indices.copy_(other.indices)
+        elif change == "permute_perm":
+            p = torch.randperm(L.in_features, generator=torch.Generator().manual_seed(1)).cuda()
+            m.perm.copy_(m.perm[p])
+        else:
+            m.load_state_dict(other.state_dict())
+        fresh = fresh_of(m, L).set_batched_decode(True)
+        for t in (2, 5, 8):
+            x = xs(L, t, seed=80 + t)
+            assert_route("batch", lambda: m(x))
+            y = m(x)
+            assert same(y, fresh(x)), (change, t)
+            close64(layer_of(m, L), x, y)
+    heads_at_rest()
+
+
+def test_batch_load_state_dict_through_fuse():
+    import vptq_b200
+    p = QKV()
+    vptq_b200.fuse(p)
+    vptq_b200.set_batched_decode(p)
+    x5 = xs(layer("q"), 5, seed=5)
+    with torch.no_grad():
+        p(x5)
+    sd = {**{"q_proj." + k: v for k, v in make_module(layer("other_q")).state_dict().items()},
+          **{"k_proj." + k: v for k, v in p.k_proj.layer.state_dict().items()},
+          **{"v_proj." + k: v for k, v in p.v_proj.layer.state_dict().items()}}
+    p.load_state_dict(sd)
+    fresh = fresh_qkv([make_module(layer("other_q")), p.k_proj.layer, p.v_proj.layer])
+    vptq_b200.set_batched_decode(fresh)
+    with torch.no_grad():
+        y = p(x5)                                    # rebuilds q_proj's descriptor and lists
+        assert_route("batch", lambda: p(x5))
+        assert same(y, fresh(x5))
+    close64(layer("other_q"), x5, y[:, :264])
+    heads_at_rest()
+
+
+def test_batch_under_inference_mode():
+    """C1 / C2: a module and a fused group under torch.inference_mode(), a graph included, equal to no_grad"""
+    import vptq_b200
+    L = layer("lists_bf16")
+    m = batched(L)
+    p = QKV()
+    vptq_b200.fuse(p)
+    vptq_b200.set_batched_decode(p)
+    x, xq = xs(L, 7, seed=7), xs(layer("q"), 4, seed=4)
+    with torch.no_grad():
+        ref, refq = m(x), p(xq)
+    with torch.inference_mode():
+        xi, xqi = x.clone(), xq.clone()
+        assert_route("batch", lambda: m(xi))
+        assert_route("batch", lambda: p(xqi))
+        got, gotq = m(xi), p(xqi)
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            m(xi)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=s):
+                yg = m(xi)
+            g.replay()
+        torch.cuda.synchronize()
+    assert same(got, ref) and same(yg, ref) and same(gotq, refq)
+    close64(L, x, got)
+    qkv_oracle_check(xq, gotq)
+    heads_at_rest()
+
+
+# ------------------------------------------------------------------------------------------------ PDL chain
+def test_batch_pdl_chain_of_a_llama_decoder_layer():
+    """Llama-3-8B decoder layer of batched launches, each with programmatic dependent launch and reading the previous
+    launch's output view directly: q/k/v -> o (on the q slice) -> gate/up -> down (on the gate slice) -> the next
+    q/k/v.  Eager and as one CUDA graph, every stage the bits of the same launches run one at a time without PDL,
+    and within the bar on the x it consumed"""
+    from _batch import GpuLayer, assert_close, kernel_star, q_of
+    from vptq_b200 import native
+    qkv = [GpuLayer(4096, o, seed=90 + k) for k, o in enumerate((4096, 1024, 1024))]
+    o_proj = [GpuLayer(4096, 4096, seed=93)]
+    gate_up = [GpuLayer(4096, 14336, seed=94 + k) for k in range(2)]
+    down = [GpuLayer(14336, 4096, seed=96)]
+    qkv2 = [GpuLayer(4096, o, seed=97 + k) for k, o in enumerate((4096, 1024, 1024))]
+    stages = [qkv, o_proj, gate_up, down, qkv2]
+    for tokens in (2, 5, 8):
+        x0 = torch.randn(tokens, 4096, device="cuda", generator=torch.Generator(device="cuda").manual_seed(tokens))
+        x0 = (0.5 * x0).half()
+        outs = [torch.empty(tokens, sum(l.O for l in st), dtype=torch.float16, device="cuda") for st in stages]
+
+        def views(k):
+            a, v = 0, []
+            for l in stages[k]:
+                v.append(outs[k][:, a:a + l.O])
+                a += l.O
+            return v
+        srcs = [x0, outs[0][:, :4096], outs[1], outs[2][:, :14336], outs[3]]
+        launches = [native.FusedGemvBatch([l.desc for l in st], views(k)) for k, st in enumerate(stages)]
+
+        def chain(flags):
+            for fb, src in zip(launches, srcs):
+                fb(src, flags)
+
+        ref = []
+        for fb, src, out in zip(launches, srcs, outs):          # one at a time, no PDL
+            fb(src, 0)
+            torch.cuda.synchronize()
+            ref.append(out.clone())
+        for o in outs:
+            o.fill_(float("nan"))
+        chain(native.FLAG_PDL)
+        torch.cuda.synchronize()
+        assert all(same(o, r) for o, r in zip(outs, ref)), tokens
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            chain(native.FLAG_PDL)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=s):
+                chain(native.FLAG_PDL)
+        for o in outs:
+            o.fill_(float("nan"))
+        for _ in range(3):
+            g.replay()
+        torch.cuda.synchronize()
+        for k, (o, r) in enumerate(zip(outs, ref)):
+            assert same(o, r), (tokens, k)
+        for k, st in enumerate(stages):
+            src = x0 if k == 0 else [None, ref[0][:, :4096], ref[1], ref[2][:, :14336], ref[3]][k]
+            a = 0
+            for l in st:
+                rows = l.sample(16, seed=k)
+                Ls, cols, keep = l.oracle(rows)
+                idx = torch.from_numpy(np.nonzero(keep)[0]).cuda()
+                ys = ref[k][:, a:a + l.O][:, torch.from_numpy(cols[keep]).cuda()]
+                assert_close(ys, kernel_star(Ls, src)[:, idx], l.dtype, q_of(l.I, l.K))
+                a += l.O
+        del g
+    heads_at_rest()

@@ -90,6 +90,33 @@ def test_gemv_matches_reference_cuda(ref, name):
         assert e_mut <= max(tol, 2 * e_ref), (e_mut, e_ref)
 
 
+@pytest.mark.parametrize("name", ["llama3_k65536_r256", "k65536_r0", "bf16"])
+def test_batched_decode_matches_reference_cuda(ref, name):
+    """the batched list kernel (2 tokens, one launch) against the same record, with the same bars"""
+    import torch
+    from _batch import BATCH, batch, desc_of
+    from _gpu import from_t, x_to_t
+    from _probe import launched_kernels, ran
+    L = vo.make_layer(seed=GEMV_SEED, **CASES[name])
+    d = desc_of(L)
+    tol = 1e-3 if L.dtype == "fp16" else 8e-3
+    x_np = vo.make_x(2, L.in_features, L.dtype, seed=2)
+    x = x_to_t(x_np, L)
+    out = [torch.empty(2, L.out_features, dtype=x.dtype, device="cuda")]
+    names = launched_kernels(lambda: batch(d, x, out))
+    assert len(names) == 1 and ran(names, BATCH), names
+    torch.cuda.synchronize()
+    y_ours = from_t(out[0])
+    y_ref = from_bits(ref[f"gemv__{name}__t2"], L.dtype)
+    y_star = vo.quant_gemm(x_np, L)
+    e_ours = parity_error(y_ours, y_star)
+    assert e_ours <= tol
+    assert np.isfinite(y_ref).all() and y_ours.shape == y_ref.shape
+    e_ref, e_mut = parity_error(y_ref, y_star), parity_error(y_ours, y_ref)
+    print(f"{name} batched x2: ours-vs-exact {e_ours:.2e}  ref-vs-exact {e_ref:.2e}  ours-vs-ref {e_mut:.2e}")
+    assert e_mut <= max(tol, 2 * e_ref), (e_mut, e_ref)
+
+
 @pytest.mark.parametrize("name", DEQUANT_CASES)
 def test_dequant_matches_reference_cuda(ref, name):
     from _gpu import from_t, make_module
