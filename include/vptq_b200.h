@@ -100,7 +100,9 @@ typedef struct vptq_linear_desc {
      field j of a row = bits [j*b, (j+1)*b) of its little-endian bit stream,
      field = idx | ridx << ib   (vptq/utils/pack.py:41-67).  Strides in 32-bit words. */
   const int32_t* indices; /* may be NULL when lists_stream / lists_tab are given (decode-only descriptor: the packed
-                             words were dropped after the lists were built; only single-token GEMV calls work) */
+                             words were dropped after the lists were built; the calls of this header then take single
+                             tokens only, include/vptq_b200_batch.h 1..8 tokens, and include/vptq_b200_lists_dense.h
+                             prefill, dequant and the input gradient) */
   int64_t index_stride_codebook;
   int64_t index_stride_row;
 
@@ -351,6 +353,7 @@ VPTQ_B200_API int vptq_b200_linear_host(const vptq_linear_desc* desc, const void
 
 /* Workspace helpers for hosts that capture CUDA graphs: include/vptq_b200_graph.h. */
 /* Batched decode (2..8 tokens) from the index lists: include/vptq_b200_batch.h. */
+/* Prefill, dequant and input gradient from the index lists (decode-only descriptors): include/vptq_b200_lists_dense.h. */
 
 #ifdef __cplusplus
 }

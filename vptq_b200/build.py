@@ -20,7 +20,7 @@ INCLUDE = os.path.join(os.path.dirname(HERE), "include")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libvptq_b200.so")
 
-SOURCES = ["api.cu", "gemv.cu", "gemv_inst_v8.cu", "gemv_inst_vx.cu", "gemv_lists.cu", "gemv_lists_batch.cu", "lists_build.cu", "dequant.cu", "gemv_v2.cu", "gemm_wgmma.cu", "wgrad.cu"]
+SOURCES = ["api.cu", "gemv.cu", "gemv_inst_v8.cu", "gemv_inst_vx.cu", "gemv_lists.cu", "gemv_lists_batch.cu", "lists_build.cu", "lists_dense.cu", "dequant.cu", "gemv_v2.cu", "gemm_wgmma.cu", "wgrad.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = (["-DVPTQ_B200_PROF_WARPS"] if os.environ.get("VPTQ_B200_PROF_WARPS") else []) + [*ARCH, "-lineinfo", "-O3", "-std=c++17",
@@ -43,6 +43,7 @@ def _headers():
     hs.append(os.path.join(INCLUDE, "vptq_b200_grad.h"))
     hs.append(os.path.join(INCLUDE, "vptq_b200_graph.h"))
     hs.append(os.path.join(INCLUDE, "vptq_b200_batch.h"))
+    hs.append(os.path.join(INCLUDE, "vptq_b200_lists_dense.h"))
     return hs
 
 

@@ -157,6 +157,26 @@ int need_packed(const vptq_linear_desc* d, const char* what) {
   return VPTQ_ERR_UNSUPPORTED;
 }
 
+// calls of include/vptq_b200_lists_dense.h: a descriptor whose index lists the list kernels take, full or decode-only
+int validate_lists(const vptq_linear_desc* d, uint32_t flags, uint32_t allowed_flags, const char* what) {
+  if (int rc = validate(d, false)) return rc;
+  if (flags & ~allowed_flags) {
+    set_error("%s: unknown flags 0x%x", what, flags);
+    return VPTQ_ERR_INVALID;
+  }
+  if (!d->lists_stream || !d->lists_tab) {
+    set_error("%s: this descriptor carries no index lists (lists_stream / lists_tab are NULL)", what);
+    return VPTQ_ERR_UNSUPPORTED;
+  }
+  if (!gemv_lists_eligible(*d)) {
+    set_error("%s: index lists of a layer the list kernels do not take (vector_len 8, one codebook group, no outliers, "
+              "K = 4096 * (2..16), Kr <= 256, lists_tile_cols of the lists geometry, 16-byte aligned lists_stream, "
+              "weight_scale and weight_bias)", what);
+    return VPTQ_ERR_UNSUPPORTED;
+  }
+  return 0;
+}
+
 // the gradient outputs must match tensors the layer has, 16-bit aligned
 int validate_grads(const vptq_linear_desc* d, const vptq_linear_grads* g, uint32_t flags, uint32_t allowed_flags,
                    const char* what) {
@@ -530,6 +550,45 @@ int vptq_b200_quant_gemv_batch(int32_t n, const vptq_linear_desc* const* descs, 
   }
   return gemv_lists_batch_launch(n, descs, x, x_stride, ys, y_strides, tokens, flags, static_cast<cudaStream_t>(stream),
                                  workspace, workspace_bytes);
+}
+
+// ---- prefill, dequant and input gradient from the index lists (include/vptq_b200_lists_dense.h) ----
+int vptq_b200_lists_dense_version(void) { return VPTQ_B200_LISTS_DENSE_VERSION; }
+
+size_t vptq_b200_lists_dense_workspace_bytes(const vptq_linear_desc* desc, int32_t tokens, uint32_t flags) {
+  if (validate_lists(desc, flags, VPTQ_FLAG_TRANSPOSE | VPTQ_FLAG_PDL, "lists_dense_workspace_bytes")) return 0;
+  if (tokens < 1) tokens = 1;
+  return lists_gemm_workspace_bytes(*desc, tokens, (flags & VPTQ_FLAG_TRANSPOSE) != 0);
+}
+
+int vptq_b200_lists_dequant(const vptq_linear_desc* desc, void* w, int64_t ld, uint32_t flags, void* stream) {
+  if (int rc = validate_lists(desc, flags, VPTQ_FLAG_TRANSPOSE, "lists_dequant")) return rc;
+  const bool tr = (flags & VPTQ_FLAG_TRANSPOSE) != 0;
+  const int cols = tr ? desc->out_features : desc->in_features;
+  if (!w || (reinterpret_cast<uintptr_t>(w) & 15u) || ld < cols || (ld % 8)) {
+    set_error("lists_dequant: w must be 16-byte aligned and ld (%lld) a multiple of 8 >= %s (%d)", (long long)ld,
+              tr ? "out_features" : "in_features", cols);
+    return VPTQ_ERR_INVALID;
+  }
+  if (int rc = check_device()) return rc;
+  return lists_dense_launch(*desc, w, ld, tr, static_cast<cudaStream_t>(stream));
+}
+
+int vptq_b200_lists_quant_gemm(const vptq_linear_desc* desc, const void* x, int64_t x_stride, void* y,
+                               int64_t y_stride, int32_t tokens, void* workspace, size_t workspace_bytes,
+                               uint32_t flags, void* stream) {
+  if (int rc = validate_lists(desc, flags, VPTQ_FLAG_TRANSPOSE | VPTQ_FLAG_PDL, "lists_quant_gemm")) return rc;
+  const bool tr = (flags & VPTQ_FLAG_TRANSPOSE) != 0;
+  const int xcols = tr ? desc->out_features : desc->in_features, ycols = tr ? desc->in_features : desc->out_features;
+  if (!x || !y || tokens < 1 || x_stride < xcols || y_stride < ycols || (reinterpret_cast<uintptr_t>(x) & 1u) ||
+      (reinterpret_cast<uintptr_t>(y) & 1u)) {
+    set_error("lists_quant_gemm%s: bad x/y/tokens/strides (tokens %d, x_stride %lld must be >= %d, y_stride %lld >= "
+              "%d)", tr ? " (transpose)" : "", tokens, (long long)x_stride, xcols, (long long)y_stride, ycols);
+    return VPTQ_ERR_INVALID;
+  }
+  if (int rc = check_device()) return rc;
+  return lists_gemm_launch(*desc, x, x_stride, y, y_stride, tokens, workspace, workspace_bytes, tr,
+                           static_cast<cudaStream_t>(stream));
 }
 
 int vptq_b200_stream_capture_id(void* stream, uint64_t* id) {

@@ -679,6 +679,88 @@ int gemm_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void
   return 0;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Prefill and input gradient with the weight written from the index lists (lists_dense.cu, C interface
+// include/vptq_b200_lists_dense.h).  Forward: W [O][kpad] in original feature order, scale / weight_bias folded in --
+// the B operand of gemm_launch's prep-free route -- and x handed to TMA as it is when its rows are 16-byte aligned
+// whole BK blocks, otherwise staged to [T][kpad] with zero K padding; bias in the epilogue.  Transposed: Wt [I][ld]
+// and dY exactly as in dgrad_launch.  Both tensor maps are encoded before anything is launched.
+// ---------------------------------------------------------------------------------------------
+namespace {
+
+struct ListsGemmWorkspace {
+  size_t off_w, off_x, total;
+  int64_t ld;  // pitch of W (kpad) or Wt and of the staged activation
+};
+ListsGemmWorkspace lists_gemm_layout(const vptq_linear_desc& d, int tokens, bool transposed) {
+  ListsGemmWorkspace w;
+  if (transposed) {
+    const DgradWorkspace g = dgrad_layout(d, tokens);
+    w.off_w = g.off_wt, w.off_x = g.off_dy, w.total = g.total, w.ld = g.ld;
+    return w;
+  }
+  w.ld = int64_t(align_up(size_t(d.in_features), 64));
+  size_t off = kZeroRegionBytes;  // the zero-at-rest region stays untouched
+  w.off_w = off;
+  off += align_up(size_t(d.out_features) * w.ld * 2, 1024);
+  w.off_x = off;
+  off += align_up(size_t(tokens) * w.ld * 2, 1024);
+  w.total = off;
+  return w;
+}
+
+}  // namespace
+
+size_t lists_gemm_workspace_bytes(const vptq_linear_desc& d, int tokens, bool transposed) {
+  return lists_gemm_layout(d, tokens, transposed).total;
+}
+
+int lists_gemm_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void* y, int64_t y_stride, int tokens,
+                      void* workspace, size_t workspace_bytes, bool transposed, cudaStream_t stream) {
+  const char* what = transposed ? "lists_quant_gemm (transpose)" : "lists_quant_gemm";
+  const ListsGemmWorkspace w = lists_gemm_layout(d, tokens, transposed);
+  if (!workspace || workspace_bytes < w.total) {
+    set_error("%s: workspace %zu bytes < required %zu", what, workspace_bytes, w.total);
+    return VPTQ_ERR_WORKSPACE;
+  }
+  uint8_t* ws = reinterpret_cast<uint8_t*>(workspace);
+  void* wd = ws + w.off_w;
+  const int is_bf16 = d.dtype == VPTQ_BF16;
+  const int K = transposed ? d.out_features : d.in_features;  // valid extent of the reduction
+  const int N = transposed ? d.in_features : d.out_features;
+  const bool stage = int64_t(K) != w.ld || (reinterpret_cast<uintptr_t>(x) & 15u) || (x_stride % 8);
+  const void* a = stage ? static_cast<const void*>(ws + w.off_x) : x;
+  const int64_t a_ld = stage ? w.ld : x_stride;
+  CUtensorMap map_a, map_b;
+  if (int rc = make_map(&map_a, is_bf16, a, tokens, w.ld, a_ld, BM)) return rc;
+  if (int rc = make_map(&map_b, is_bf16, wd, N, w.ld, w.ld, BN)) return rc;
+  const DeviceInfo* dev = device_info();
+  if (!dev) return VPTQ_ERR_CUDA;
+  const void* fn = is_bf16 ? reinterpret_cast<const void*>(gemm_tn_wgmma<__nv_bfloat16>)
+                           : reinterpret_cast<const void*>(gemm_tn_wgmma<__half>);
+  if (int rc = ensure_smem_attr(fn, GEMM_SMEM)) return rc;
+
+  if (int rc = lists_dense_launch(d, wd, w.ld, transposed, stream)) return rc;
+  if (stage)
+    dgrad_stage_dy<<<tokens, 256, 0, stream>>>(reinterpret_cast<const uint16_t*>(x), x_stride,
+                                                reinterpret_cast<uint16_t*>(ws + w.off_x), w.ld, K);
+  GemmParams p{};
+  p.bias = transposed ? nullptr : d.bias, p.rowbias = nullptr, p.y = y, p.y_stride = y_stride;
+  p.T = tokens, p.O = N, p.K = int(w.ld), p.is_bf16 = is_bf16;
+  const int ntiles = ((N + BN - 1) / BN) * ((tokens + BM - 1) / BM);
+  dim3 grid(unsigned(std::min(ntiles, dev->sm_count)));  // persistent: one CTA per SM
+  if (is_bf16)
+    gemm_tn_wgmma<__nv_bfloat16><<<grid, GEMM_THREADS, GEMM_SMEM, stream>>>(map_a, map_b, p);
+  else
+    gemm_tn_wgmma<__half><<<grid, GEMM_THREADS, GEMM_SMEM, stream>>>(map_a, map_b, p);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    set_error("%s launch: %s", what, cudaGetErrorString(e));
+    return VPTQ_ERR_CUDA;
+  }
+  return 0;
+}
+
 int wgrad_gamma_launch(int is_bf16, const void* a, const void* b, int M, int N, int K, float* gamma, int64_t ld,
                        cudaStream_t stream) {
   if ((N & 1) || (ld & 1) || ld < N || (K % BK) || (reinterpret_cast<uintptr_t>(gamma) & 7u)) {

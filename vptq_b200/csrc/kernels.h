@@ -9,6 +9,7 @@
 #include "../../include/vptq_b200_grad.h"
 #include "../../include/vptq_b200_graph.h"
 #include "../../include/vptq_b200_batch.h"
+#include "../../include/vptq_b200_lists_dense.h"
 
 namespace vptq_b200 {
 
@@ -125,6 +126,10 @@ bool dequant_orig_fast_ok(const vptq_linear_desc& d, const void* w_out, int64_t 
 // Wt[f][o] = W[o][f], rows in original feature order, pitch ld (multiple of 8, >= out_features), columns [O, ld) zero
 int dequant_transposed_launch(const vptq_linear_desc& d, void* wt_out, int64_t ld, cudaStream_t stream);
 
+// the same W (transposed: Wt) from the index lists (lists_dense.cu, C interface include/vptq_b200_lists_dense.h):
+// layers with gemv_lists_eligible(d), out 16-byte aligned, ld % 8 == 0, ld >= in_features (Wt: >= out_features)
+int lists_dense_launch(const vptq_linear_desc& d, void* out, int64_t ld, bool transposed, cudaStream_t stream);
+
 // -------------------------------------------------------------------------------------------
 // prefill GEMM (wgmma)
 // -------------------------------------------------------------------------------------------
@@ -135,6 +140,10 @@ int gemm_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void
 size_t dgrad_workspace_bytes(const vptq_linear_desc& d, int tokens);
 int dgrad_launch(const vptq_linear_desc& d, const void* dy, int64_t dy_stride, void* dx, int64_t dx_stride, int tokens,
                  void* workspace, size_t workspace_bytes, cudaStream_t stream);
+// prefill (transposed: input gradient) with W (Wt) written from the index lists instead of the packed words
+size_t lists_gemm_workspace_bytes(const vptq_linear_desc& d, int tokens, bool transposed);
+int lists_gemm_launch(const vptq_linear_desc& d, const void* x, int64_t x_stride, void* y, int64_t y_stride, int tokens,
+                      void* workspace, size_t workspace_bytes, bool transposed, cudaStream_t stream);
 // gamma[M][ld] (fp32, unrounded) = A[M][K] . B[N][K]^T with both operands K-major, K % 64 == 0, N and ld even
 int wgrad_gamma_launch(int is_bf16, const void* a, const void* b, int M, int N, int K, float* gamma, int64_t ld,
                        cudaStream_t stream);

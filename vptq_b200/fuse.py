@@ -19,6 +19,10 @@ index lists (`VQuantLinear.prepare`), so nothing is allocated or re-bucketed ins
 
 After `set_batched_decode(model)` a group whose members all opted in also launches 2..8-token activations as one
 batched list-kernel launch (include/vptq_b200_batch.h), with the same results as its members' own forwards.
+
+`set_lists_prefill(model)` lets decode-only layers (`prepare(drop_packed=True)`) serve prompts from their index lists
+(include/vptq_b200_lists_dense.h).  The generic fused launch cannot take 2-token calls of such a group, so those go to
+each member's own forward.
 """
 from __future__ import annotations
 
@@ -30,7 +34,8 @@ import torch.nn as nn
 from . import native
 from .layers import VQuantLinear
 
-__all__ = ["fuse", "unfuse", "set_quant_grad", "set_batched_decode", "FusedGroup", "FusedMember", "DEFAULT_GROUPS"]
+__all__ = ["fuse", "unfuse", "set_quant_grad", "set_batched_decode", "set_lists_prefill", "FusedGroup", "FusedMember",
+           "DEFAULT_GROUPS"]
 
 DEFAULT_GROUPS: Tuple[Tuple[str, ...], ...] = (("q_proj", "k_proj", "v_proj"), ("gate_proj", "up_proj"))
 
@@ -77,6 +82,10 @@ class FusedGroup:
         batched = tokens >= 2 and all(getattr(l, "_batched_decode", False) for l in self.layers)
         if tokens > 2 and not batched:
             return None
+        # decode-only members (set_lists_prefill) route 2-token calls the batched kernel does not take themselves
+        lists_member = tokens == 2 and any(getattr(l, "_lists_prefill", False) and l._decode_only() for l in self.layers)
+        if lists_member and not batched:
+            return None
         key = activation_key(x)
         if key == self._key and self._out is not None and not (self._served >> index) & 1:
             self._served |= 1 << index
@@ -85,7 +94,7 @@ class FusedGroup:
             return self._out
         descs = self._descs(x)
         if batched and (x2.data_ptr() % 16 or tokens > native.batch_max_tokens(descs)):
-            if tokens > 2:
+            if tokens > 2 or lists_member:
                 return None       # each member routes its own call (its own batched launch where it is eligible)
             batched = False
         fkey = tuple(id(d) for d in descs) + (tokens, batched)
@@ -209,6 +218,16 @@ def set_batched_decode(model: nn.Module, enabled: bool = True) -> int:
     layers = [l for l in layers if isinstance(l, VQuantLinear)]
     for l in layers:
         l.set_batched_decode(enabled)
+    return len(layers)
+
+
+def set_lists_prefill(model: nn.Module, enabled: bool = True) -> int:
+    """`VQuantLinear.set_lists_prefill(enabled)` on every VQuantLinear of `model`, fused members included.  Returns
+    how many layers it reached."""
+    layers = [mod.layer if isinstance(mod, FusedMember) else mod for mod in model.modules()]
+    layers = [l for l in layers if isinstance(l, VQuantLinear)]
+    for l in layers:
+        l.set_lists_prefill(enabled)
     return len(layers)
 
 

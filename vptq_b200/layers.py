@@ -26,7 +26,7 @@ import torch
 import torch.nn as nn
 from torch.nn.parameter import Parameter
 
-from . import ops
+from . import native, ops
 from .pack import pack_index
 
 __all__ = ["VQuantLinear"]
@@ -55,7 +55,8 @@ class VQuantLinear(nn.Module):
     (see `set_centroids_grad`) decides which ones are computed; they come out in the parameter's dtype, summed in
     64-bit fixed point and rounded once, bit-identical from run to run (include/vptq_b200_grad.h).  Without the
     opt-in they get no gradient, as with the reference's CUDA extension.  Indices and perm never get one.  There is
-    no double backward, and the backward of a decode-only module (`prepare(drop_packed=True)`) raises."""
+    no double backward, and the backward of a decode-only module (`prepare(drop_packed=True)`) raises unless it opted
+    in with `set_lists_prefill()` (input and bias gradients only)."""
 
     def __init__(
         self,
@@ -163,6 +164,7 @@ class VQuantLinear(nn.Module):
         self._packed = None              # lazily packed indices for unpacked checkpoints
         self._quant_grad = False         # set_quant_grad
         self._batched_decode = False     # set_batched_decode
+        self._lists_prefill = False      # set_lists_prefill
 
     # ------------------------------------------------------------------------------------------
     def _tensors(self):
@@ -233,6 +235,21 @@ class VQuantLinear(nn.Module):
         self._batched_decode = bool(enabled)
         return self
 
+    def set_lists_prefill(self, enabled: bool = True) -> "VQuantLinear":
+        """Opt in to prefill, `dequant()` and the input gradient of a decode-only module (`prepare(drop_packed=True)`)
+        from its index lists: the dense weight is written from the lists into the GEMM's workspace instead of from
+        the packed words, which stay freed (include/vptq_b200_lists_dense.h).  Routing with the opt-in: 1 token ->
+        the list kernel; 2..8 tokens -> the batched list kernel where `set_batched_decode` is on and it takes the
+        call; every other call -> the GEMM from the lists.  The weight is bit-identical to the packed dequant's, so
+        `dequant()`, the input gradient and prefill calls that a full module serves by its prep-free GEMM give the
+        full module's results bit for bit.  On a module that still has its packed words nothing changes.  Weight
+        gradients (`set_quant_grad`) and saving the state_dict stay refused on a decode-only module."""
+        self._lists_prefill = bool(enabled)
+        return self
+
+    def _decode_only(self) -> bool:
+        return getattr(self, "_drop_packed", False) and self.indices.numel() == 0
+
     def _check_quant_grad_possible(self) -> None:
         if getattr(self, "_drop_packed", False) and self.indices.numel() == 0:
             raise RuntimeError("set_quant_grad: this VQuantLinear is decode-only (prepare(drop_packed=True)); the "
@@ -261,7 +278,8 @@ class VQuantLinear(nn.Module):
 
         drop_packed=True makes the module DECODE-ONLY: once the index lists exist the packed `indices` are freed
         (4.2 instead of 7.2 bytes per index resident).  Calls with more than one token, `dequant()` and saving the
-        state_dict are no longer possible; reloading a checkpoint restores them."""
+        state_dict are no longer possible; reloading a checkpoint restores them.  `set_lists_prefill()` brings back
+        multi-token calls, `dequant()` and the input gradient, computed from the lists."""
         if rebuild:
             if getattr(self, "_drop_packed", False) and self.indices.numel() == 0:
                 raise RuntimeError("prepare(rebuild=True): this VQuantLinear is decode-only (prepare(drop_packed="
@@ -337,11 +355,16 @@ class VQuantLinear(nn.Module):
             padding=self.padding, outlier_padding=self.outlier_padding,
             vector_quant_dim=self.vector_quant_dim, _desc_cache=self._desc_cache,
             _drop_packed=getattr(self, "_drop_request", False), _quant_grad=getattr(self, "_quant_grad", False),
-            _batched_decode=getattr(self, "_batched_decode", False))
+            _batched_decode=getattr(self, "_batched_decode", False),
+            _lists_prefill=getattr(self, "_lists_prefill", False))
 
     def dequant(self) -> torch.Tensor:
-        """Dense [out_features, in_features] weight through the CUDA dequant kernel."""
-        if getattr(self, "_drop_packed", False) and self.indices.numel() == 0:
+        """Dense [out_features, in_features] weight through the CUDA dequant kernel (from the index lists on a
+        decode-only module with `set_lists_prefill()`)."""
+        if self._decode_only() and getattr(self, "_lists_prefill", False) and self._desc_cache:
+            cent = self.centroids.weight
+            return native.lists_dense_weight(self._desc_cache[0], cent.dtype, cent.device)
+        if self._decode_only():
             raise RuntimeError("this VQuantLinear is decode-only (prepare(drop_packed=True)): the packed index words "
                                "dequant needs were freed; reload the checkpoint to get them back")
         indices, cent, resc, outi, outc, perm, ws, wb, _ = self._tensors()

@@ -47,6 +47,11 @@ GRAD_FLAG_GENERIC = 1
 BATCH_EXPORTS = ("vptq_b200_batch_version", "vptq_b200_quant_gemv_batch_max_tokens", "vptq_b200_quant_gemv_batch")
 BATCH_VERSION = 1
 
+# prefill, dequant and input gradient from the index lists (include/vptq_b200_lists_dense.h), same library
+LISTS_DENSE_EXPORTS = ("vptq_b200_lists_dense_version", "vptq_b200_lists_dense_workspace_bytes",
+                       "vptq_b200_lists_dequant", "vptq_b200_lists_quant_gemm")
+LISTS_DENSE_VERSION = 1
+
 MAX_FUSED, MAX_RANKS = 4, 8
 
 
@@ -174,6 +179,19 @@ def lib() -> ctypes.CDLL:
         L.vptq_b200_quant_gemv_batch.restype = ctypes.c_int
         if L.vptq_b200_batch_version() != BATCH_VERSION:
             raise RuntimeError(f"libvptq_b200.so batch interface {L.vptq_b200_batch_version()} != expected {BATCH_VERSION}")
+        for f in LISTS_DENSE_EXPORTS:
+            if not hasattr(L, f):
+                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_lists_dense.h): rebuild it")
+        L.vptq_b200_lists_dense_version.restype = ctypes.c_int
+        L.vptq_b200_lists_dense_workspace_bytes.argtypes = [dp, i32, u32]
+        L.vptq_b200_lists_dense_workspace_bytes.restype = ctypes.c_size_t
+        L.vptq_b200_lists_dequant.argtypes = [dp, vp, i64, u32, vp]
+        L.vptq_b200_lists_dequant.restype = ctypes.c_int
+        L.vptq_b200_lists_quant_gemm.argtypes = [dp, vp, i64, vp, i64, i32, vp, sz, u32, vp]
+        L.vptq_b200_lists_quant_gemm.restype = ctypes.c_int
+        if L.vptq_b200_lists_dense_version() != LISTS_DENSE_VERSION:
+            raise RuntimeError(f"libvptq_b200.so lists-dense interface {L.vptq_b200_lists_dense_version()} != expected "
+                               f"{LISTS_DENSE_VERSION}")
         _lib = L
     return _lib
 
@@ -558,6 +576,48 @@ def quant_gemm_dgrad(desc: LinearDesc, dy2d: torch.Tensor, dx2d: torch.Tensor) -
         rc = lib().vptq_b200_quant_gemm(ctypes.byref(desc), dy2d.data_ptr(), row_pitch(dy2d), dx2d.data_ptr(),
                                         row_pitch(dx2d), tokens, ws.data_ptr(), ws.numel(), FLAG_TRANSPOSE, _stream(dev))
     check(rc, "vptq_b200_quant_gemm (transpose)")
+
+
+def lists_dense_workspace_bytes(desc: LinearDesc, tokens: int, flags: int = 0) -> int:
+    return int(lib().vptq_b200_lists_dense_workspace_bytes(ctypes.byref(desc), int(tokens), int(flags)))
+
+
+def lists_quant_gemm(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, flags: int = 0) -> None:
+    """vptq_b200_lists_quant_gemm: y2d = x2d @ W^T + bias (flags 0) or the input gradient y2d = x2d @ W with x2d = dY
+    (FLAG_TRANSPOSE), the weight written from the index lists.  Any token count >= 1."""
+    x2d = _dense_rows(x2d)
+    tokens = x2d.shape[0]
+    dev = x2d.device
+    with _on_device(dev):
+        cache = desc.__dict__.setdefault("_lists_ws", {})
+        key = (tokens, flags & FLAG_TRANSPOSE)
+        nbytes = cache.get(key)
+        if nbytes is None:
+            nbytes = cache[key] = lists_dense_workspace_bytes(desc, tokens, flags)
+        ws = workspace(dev, max(nbytes, 1))
+        rc = lib().vptq_b200_lists_quant_gemm(ctypes.byref(desc), x2d.data_ptr(), row_pitch(x2d), y2d.data_ptr(),
+                                              row_pitch(y2d), tokens, ws.data_ptr(), ws.numel(), int(flags),
+                                              _stream(dev))
+    check(rc, "vptq_b200_lists_quant_gemm" + (" (transpose)" if flags & FLAG_TRANSPOSE else ""))
+
+
+def lists_dequant(desc: LinearDesc, w: torch.Tensor, ld: int, flags: int = 0) -> None:
+    """vptq_b200_lists_dequant into the buffer starting at w: W [out_features][ld] (flags 0) or Wt [in_features][ld]
+    (FLAG_TRANSPOSE), written from the index lists; ld a multiple of 8, columns past the weight's zero."""
+    dev = w.device
+    with _on_device(dev):
+        rc = lib().vptq_b200_lists_dequant(ctypes.byref(desc), w.data_ptr(), int(ld), int(flags), _stream(dev))
+    check(rc, "vptq_b200_lists_dequant")
+
+
+def lists_dense_weight(desc: LinearDesc, dtype: torch.dtype, device) -> torch.Tensor:
+    """The layer's dense weight [out_features, in_features] from the index lists (a view into rows padded to a
+    multiple of 8 elements when in_features is not one)."""
+    I, O = desc.in_features, desc.out_features
+    ld = (I + 7) // 8 * 8
+    buf = torch.empty(O, ld, dtype=dtype, device=device)
+    lists_dequant(desc, buf, ld)
+    return buf if ld == I else buf[:, :I]
 
 
 def grad_workspace_bytes(desc: LinearDesc, tokens: int, op: int) -> int:

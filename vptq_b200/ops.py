@@ -8,7 +8,10 @@ Function names, argument order and argument meaning are the reference's
   torch implementation to fall back to -- CPU tensors raise;
 * routing: fewer than 3 tokens -> fused GEMV (the reference's rule, :213); otherwise the fused
   dequant->wgmma GEMM instead of `dequant` + `F.linear` (:231-275).  Opt-in (`_batched_decode`,
-  VQuantLinear.set_batched_decode): 2..8 tokens of a layer with index lists -> the batched list kernel;
+  VQuantLinear.set_batched_decode): 2..8 tokens of a layer with index lists -> the batched list kernel.  Opt-in
+  (`_lists_prefill`, VQuantLinear.set_lists_prefill): a decode-only descriptor takes every call the list kernels do
+  not through the GEMM with the weight written from the index lists (include/vptq_b200_lists_dense.h), and its input
+  gradient likewise;
 * `argsort(perm)` is not recomputed on every call (the reference does, :208-211).
 """
 from __future__ import annotations
@@ -175,6 +178,7 @@ def quant_gemm(
     _drop_packed: bool = False,
     _quant_grad: bool = False,
     _batched_decode: bool = False,
+    _lists_prefill: bool = False,
 ) -> torch.Tensor:
     """y = x @ W^T + bias for one VPTQ layer (reference: vptq/ops/quant_gemm.py:161-275).
 
@@ -182,7 +186,11 @@ def quant_gemm(
     require grad get gradients too, also when x does not require grad (vptq_b200_quant_gemm_wgrad).
 
     `_batched_decode` (VQuantLinear.set_batched_decode): 2..batch_max_tokens tokens of a layer that carries index
-    lists run the batched list kernel (include/vptq_b200_batch.h); every other call is routed as without it."""
+    lists run the batched list kernel (include/vptq_b200_batch.h); every other call is routed as without it.
+
+    `_lists_prefill` (VQuantLinear.set_lists_prefill): on a decode-only descriptor, calls neither list kernel takes
+    and the input gradient run the GEMM with the weight written from the index lists; no effect on a descriptor
+    that still has its packed words."""
     if vector_quant_dim == "in":
         raise ValueError("Not implemented yet.")
     if not is_indice_packed:
@@ -223,17 +231,18 @@ def quant_gemm(
             if not quant:
                 layer = (indices, centroids, residual_centroids, outlier_indices, outlier_centroids, perm,
                          weight_scale, weight_bias)
-                y = _QuantLinearFn.apply(x2d, bias, keep, out_features, _batched_decode,
+                y = _QuantLinearFn.apply(x2d, bias, keep, out_features, (_batched_decode, _lists_prefill),
                                          *[t for t in layer if t is not None])
             else:
                 others = [t for t in (indices, outlier_indices, perm) if t is not None]
-                y = _QuantLinearWgradFn.apply(x2d, bias, keep, out_features, _batched_decode,
+                y = _QuantLinearWgradFn.apply(x2d, bias, keep, out_features, (_batched_decode, _lists_prefill),
                                               tuple(n for n, _ in slots), *[t for _, t in slots], *others)
             return y.reshape(*x.shape[:-1], out_features)
-    return _forward(desc, x2d, out_features, _batched_decode).reshape(*x.shape[:-1], out_features)
+    return _forward(desc, x2d, out_features, _batched_decode, _lists_prefill).reshape(*x.shape[:-1], out_features)
 
 
-def _forward(desc, x2d: torch.Tensor, out_features: int, batched: bool = False) -> torch.Tensor:
+def _forward(desc, x2d: torch.Tensor, out_features: int, batched: bool = False,
+             lists_prefill: bool = False) -> torch.Tensor:
     tokens = x2d.shape[0]
     y = torch.empty(tokens, out_features, dtype=x2d.dtype, device=x2d.device)
     if tokens == 0:
@@ -241,6 +250,8 @@ def _forward(desc, x2d: torch.Tensor, out_features: int, batched: bool = False) 
     if batched and tokens >= 2 and desc.lists_stream and x2d.data_ptr() % 16 == 0 and \
             tokens <= native.batch_max_tokens(desc):
         native.quant_gemv_batch(desc, x2d, y)
+    elif lists_prefill and tokens >= 2 and not desc.indices:
+        native.lists_quant_gemm(desc, x2d, y)
     elif tokens < 3:
         native.quant_gemv(desc, x2d, y)
     else:
@@ -258,10 +269,10 @@ class _QuantLinearFn(torch.autograd.Function):
     in-place update between forward and backward fails autograd's version check instead of using new weights."""
 
     @staticmethod
-    def forward(ctx, x2d, bias, keep, out_features, batched, *layer):
-        ctx.keep = keep
+    def forward(ctx, x2d, bias, keep, out_features, route, *layer):
+        ctx.keep, ctx.lists_prefill = keep, route[1]
         ctx.save_for_backward(*layer)
-        return _forward(keep[0], x2d, out_features, batched)
+        return _forward(keep[0], x2d, out_features, *route)
 
     @staticmethod
     @once_differentiable
@@ -273,14 +284,18 @@ class _QuantLinearFn(torch.autograd.Function):
 
 def _input_grads(ctx, desc, dy):
     """(dX, dbias) of y = x W^T + bias for the slots 0 and 1 that need them."""
-    if not desc.indices:
+    from_lists = not desc.indices and getattr(ctx, "lists_prefill", False)
+    if not desc.indices and not from_lists:
         raise RuntimeError("backward through a decode-only VQuantLinear (prepare(drop_packed=True)): the input "
                            "gradient needs the packed index words, which were freed; reload the checkpoint")
     dx = dbias = None
     if ctx.needs_input_grad[0]:
         dx = torch.empty(dy.shape[0], desc.in_features, dtype=dy.dtype, device=dy.device)
         if dy.shape[0]:
-            native.quant_gemm_dgrad(desc, dy, dx)
+            if from_lists:        # (set_lists_prefill) Wt written from the index lists
+                native.lists_quant_gemm(desc, dy, dx, native.FLAG_TRANSPOSE)
+            else:
+                native.quant_gemm_dgrad(desc, dy, dx)
     if ctx.needs_input_grad[1]:
         dbias = dy.float().sum(0).to(dy.dtype)
     return dx, dbias
@@ -296,10 +311,10 @@ class _QuantLinearWgradFn(torch.autograd.Function):
     autograd's version check)."""
 
     @staticmethod
-    def forward(ctx, x2d, bias, keep, out_features, batched, names, *layer):
-        ctx.keep, ctx.names = keep, names
+    def forward(ctx, x2d, bias, keep, out_features, route, names, *layer):
+        ctx.keep, ctx.names, ctx.lists_prefill = keep, names, route[1]
         ctx.save_for_backward(x2d, *layer)
-        return _forward(keep[0], x2d, out_features, batched)
+        return _forward(keep[0], x2d, out_features, *route)
 
     @staticmethod
     @once_differentiable
