@@ -354,6 +354,7 @@ VPTQ_B200_API int vptq_b200_linear_host(const vptq_linear_desc* desc, const void
 /* Workspace helpers for hosts that capture CUDA graphs: include/vptq_b200_graph.h. */
 /* Batched decode (2..8 tokens) from the index lists: include/vptq_b200_batch.h. */
 /* Prefill, dequant and input gradient from the index lists (decode-only descriptors): include/vptq_b200_lists_dense.h. */
+/* Decode (1..4 tokens) of vector-length-16 layers from lists with index rows of 16 outputs: include/vptq_b200_lists16.h. */
 
 #ifdef __cplusplus
 }

@@ -591,6 +591,41 @@ int vptq_b200_lists_quant_gemm(const vptq_linear_desc* desc, const void* x, int6
                            static_cast<cudaStream_t>(stream));
 }
 
+// ---- decode from the index lists of vector-length-16 layers (include/vptq_b200_lists16.h) ----
+int vptq_b200_lists16_version(void) { return VPTQ_B200_LISTS16_VERSION; }
+
+int vptq_b200_quant_gemv_lists16_max_tokens(int32_t n, const vptq_linear_desc* const* descs) {
+  if (!descs || n < 1 || n > VPTQ_MAX_FUSED) {
+    set_error("quant_gemv_lists16_max_tokens: NULL descs or n %d outside 1..%d", n, VPTQ_MAX_FUSED);
+    return 0;
+  }
+  for (int l = 0; l < n; ++l)
+    if (validate(descs[l], false)) return 0;
+  return gemv_lists16_max_tokens(n, descs);
+}
+
+int vptq_b200_quant_gemv_lists16(int32_t n, const vptq_linear_desc* const* descs, const void* x, int64_t x_stride,
+                                 void* const* ys, const int64_t* y_strides, int32_t tokens, void* workspace,
+                                 size_t workspace_bytes, uint32_t flags, void* stream) {
+  if (!descs || !x || !ys || !y_strides || n < 1 || n > VPTQ_MAX_FUSED) {
+    set_error("quant_gemv_lists16: NULL argument or n %d outside 1..%d", n, VPTQ_MAX_FUSED);
+    return VPTQ_ERR_INVALID;
+  }
+  if (flags & ~VPTQ_FLAG_PDL) {
+    set_error("quant_gemv_lists16: unknown flags 0x%x", flags);
+    return VPTQ_ERR_INVALID;
+  }
+  for (int l = 0; l < n; ++l) {
+    if (int rc = validate(descs[l], l == 0)) return rc;
+    if (!ys[l] || y_strides[l] < descs[l]->out_features || x_stride < descs[l]->in_features) {
+      set_error("quant_gemv_lists16: bad y / stride for layer %d", l);
+      return VPTQ_ERR_INVALID;
+    }
+  }
+  return gemv_lists16_launch(n, descs, x, x_stride, ys, y_strides, tokens, flags, static_cast<cudaStream_t>(stream),
+                             workspace, workspace_bytes);
+}
+
 int vptq_b200_stream_capture_id(void* stream, uint64_t* id) {
   if (!id) {
     set_error("stream_capture_id: NULL id");

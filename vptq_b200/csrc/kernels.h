@@ -10,6 +10,7 @@
 #include "../../include/vptq_b200_graph.h"
 #include "../../include/vptq_b200_batch.h"
 #include "../../include/vptq_b200_lists_dense.h"
+#include "../../include/vptq_b200_lists16.h"
 
 namespace vptq_b200 {
 
@@ -114,6 +115,14 @@ int gemv_lists_batch_max_tokens(int n, const vptq_linear_desc* const* descs);  /
 int gemv_lists_batch_launch(int n, const vptq_linear_desc* const* descs, const void* x, int64_t x_stride,
                             void* const* ys, const int64_t* y_strides, int tokens, uint32_t flags, cudaStream_t stream,
                             void* workspace, size_t workspace_bytes);
+
+// Vector-length-16 variant (gemv_lists16.cu, C interface include/vptq_b200_lists16.h): 1..4 tokens of layers
+// carrying lists with index rows of 16 outputs, the batched kernel's partition, the slice as two shared planes.
+bool gemv_lists16_eligible(const vptq_linear_desc& d);
+int gemv_lists16_max_tokens(int n, const vptq_linear_desc* const* descs);  // 0: not eligible (error set)
+int gemv_lists16_launch(int n, const vptq_linear_desc* const* descs, const void* x, int64_t x_stride, void* const* ys,
+                        const int64_t* y_strides, int tokens, uint32_t flags, cudaStream_t stream, void* workspace,
+                        size_t workspace_bytes);
 
 // -------------------------------------------------------------------------------------------
 // dequant

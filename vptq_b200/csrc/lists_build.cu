@@ -249,10 +249,14 @@ extern "C" int vptq_b200_lists_deal_host(uint32_t* stream_host, const uint32_t* 
   return 0;
 }
 
-extern "C" int vptq_b200_lists_build_host(const int32_t* indices_host, int64_t index_stride_row, int32_t out_features,
-                                          int32_t in_features, int32_t num_centroids, int32_t num_res_centroids,
-                                          const uint16_t* perm_host, void* stream_out, size_t stream_capacity,
-                                          uint32_t* tab_out, size_t* steps_out, int32_t* tile_cols_out) {
+namespace vptq_b200 {
+namespace {
+
+// the lists of index rows of V outputs (8: include/vptq_b200.h, 16: include/vptq_b200_lists16.h); V only sets Ro
+int lists_build_host(int V, const int32_t* indices_host, int64_t index_stride_row, int32_t out_features,
+                     int32_t in_features, int32_t num_centroids, int32_t num_res_centroids, const uint16_t* perm_host,
+                     void* stream_out, size_t stream_capacity, uint32_t* tab_out, size_t* steps_out,
+                     int32_t* tile_cols_out) {
   const int K = num_centroids, Kr = num_res_centroids > 0 ? num_res_centroids : 0, I = in_features;
   if (!indices_host || !tab_out || !steps_out || !tile_cols_out || out_features < 1 || I < 8 || I > 65535) {
     set_error("lists_build_host: NULL argument or size out of range (in_features %d)", I);
@@ -263,7 +267,7 @@ extern "C" int vptq_b200_lists_build_host(const int32_t* indices_host, int64_t i
     return VPTQ_ERR_UNSUPPORTED;
   }
   const int ib = ilog2(K), rb = Kr ? ilog2(Kr) : 0, b = ib + rb;
-  const int NS = K / kSlice, Ro = (out_features + 7) / 8;
+  const int NS = K / kSlice, Ro = (out_features + V - 1) / V;
   const int NT = (I + kTileMax - 1) / kTileMax, TCW = ((I + NT - 1) / NT + 7) / 8 * 8, Q = NS * NT;
   *tile_cols_out = TCW;
   const int64_t words = (int64_t(I) * b + 31) / 32;
@@ -340,4 +344,23 @@ extern "C" int vptq_b200_lists_build_host(const int32_t* indices_host, int64_t i
     }
   }
   return 0;
+}
+
+}  // namespace
+}  // namespace vptq_b200
+
+extern "C" int vptq_b200_lists_build_host(const int32_t* indices_host, int64_t index_stride_row, int32_t out_features,
+                                          int32_t in_features, int32_t num_centroids, int32_t num_res_centroids,
+                                          const uint16_t* perm_host, void* stream_out, size_t stream_capacity,
+                                          uint32_t* tab_out, size_t* steps_out, int32_t* tile_cols_out) {
+  return lists_build_host(8, indices_host, index_stride_row, out_features, in_features, num_centroids,
+                          num_res_centroids, perm_host, stream_out, stream_capacity, tab_out, steps_out, tile_cols_out);
+}
+
+extern "C" int vptq_b200_lists16_build_host(const int32_t* indices_host, int64_t index_stride_row, int32_t out_features,
+                                            int32_t in_features, int32_t num_centroids, int32_t num_res_centroids,
+                                            const uint16_t* perm_host, void* stream_out, size_t stream_capacity,
+                                            uint32_t* tab_out, size_t* steps_out, int32_t* tile_cols_out) {
+  return lists_build_host(16, indices_host, index_stride_row, out_features, in_features, num_centroids,
+                          num_res_centroids, perm_host, stream_out, stream_capacity, tab_out, steps_out, tile_cols_out);
 }

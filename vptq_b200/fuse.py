@@ -20,6 +20,10 @@ index lists (`VQuantLinear.prepare`), so nothing is allocated or re-bucketed ins
 After `set_batched_decode(model)` a group whose members all opted in also launches 2..8-token activations as one
 batched list-kernel launch (include/vptq_b200_batch.h), with the same results as its members' own forwards.
 
+After `set_list_decode(model)` a group of vector-length-16 layers that all opted in launches 1..4-token activations
+as one launch of the v = 16 list kernel (include/vptq_b200_lists16.h).  Without it such a group is never fused: each
+member takes its own forward.
+
 `set_lists_prefill(model)` lets decode-only layers (`prepare(drop_packed=True)`) serve prompts from their index lists
 (include/vptq_b200_lists_dense.h).  The generic fused launch cannot take 2-token calls of such a group, so those go to
 each member's own forward.
@@ -34,8 +38,8 @@ import torch.nn as nn
 from . import native
 from .layers import VQuantLinear
 
-__all__ = ["fuse", "unfuse", "set_quant_grad", "set_batched_decode", "set_lists_prefill", "FusedGroup", "FusedMember",
-           "DEFAULT_GROUPS"]
+__all__ = ["fuse", "unfuse", "set_quant_grad", "set_batched_decode", "set_lists_prefill", "set_list_decode", "FusedGroup",
+           "FusedMember", "DEFAULT_GROUPS"]
 
 DEFAULT_GROUPS: Tuple[Tuple[str, ...], ...] = (("q_proj", "k_proj", "v_proj"), ("gate_proj", "up_proj"))
 
@@ -78,6 +82,8 @@ class FusedGroup:
         tokens = x2.shape[0]
         if not x.is_cuda or tokens < 1 or x2.stride(-1) != 1 or (tokens > 1 and x2.stride(0) < x2.shape[1]):
             return None
+        if self.layers[0].vector_len == 16:
+            return self._outputs16(x, x2, index)
         # 2..8 tokens: the batched list kernel when every member opted in (set_batched_decode) and it takes them
         batched = tokens >= 2 and all(getattr(l, "_batched_decode", False) for l in self.layers)
         if tokens > 2 and not batched:
@@ -105,6 +111,33 @@ class FusedGroup:
                 offs.append(offs[-1] + w)
             fused = native.FusedGemvBatch if batched else native.FusedGemv
             self._fused = fused(descs, [self._out[:, a:b] for a, b in zip(offs[:-1], offs[1:])])
+            self._fused_key = fkey
+        self._fused(x2, self.flags)
+        self._key, self._served = key, 1 << index
+        return self._out
+
+    def _outputs16(self, x: torch.Tensor, x2: torch.Tensor, index: int) -> Optional[torch.Tensor]:
+        """outputs() of a vector-length-16 group: one launch of the v = 16 list kernel when every member opted in
+        (set_list_decode) and it takes the whole group at this token count, else None (each member's own forward)."""
+        if not all(getattr(l, "_list_decode", False) for l in self.layers):
+            return None
+        tokens = x2.shape[0]
+        key = activation_key(x)
+        if key == self._key and self._out is not None and not (self._served >> index) & 1:
+            self._served |= 1 << index
+            if self._served == (1 << len(self.layers)) - 1:
+                self._key = None
+            return self._out
+        descs = self._descs(x)
+        if x2.data_ptr() % 16 or tokens > native.lists16_max_tokens(descs):
+            return None
+        fkey = tuple(id(d) for d in descs) + (tokens, "lists16")
+        if self._fused is None or fkey != self._fused_key:
+            self._out = torch.empty(tokens, sum(self.widths), dtype=x.dtype, device=x.device)
+            offs = [0]
+            for w in self.widths:
+                offs.append(offs[-1] + w)
+            self._fused = native.FusedGemvLists16(descs, [self._out[:, a:b] for a, b in zip(offs[:-1], offs[1:])])
             self._fused_key = fkey
         self._fused(x2, self.flags)
         self._key, self._served = key, 1 << index
@@ -170,8 +203,8 @@ def _eligible(layers: Iterable[nn.Module]) -> bool:
         return False
     l0 = layers[0]
     return all(l.in_features == l0.in_features and l.centroids.weight.dtype == l0.centroids.weight.dtype and
-               l.centroids.weight.device == l0.centroids.weight.device and l.vector_len == 8 and
-               not l.enable_proxy_error for l in layers)
+               l.centroids.weight.device == l0.centroids.weight.device and l.vector_len == l0.vector_len and
+               l.vector_len in (8, 16) and not l.enable_proxy_error for l in layers)
 
 
 def fuse(model: nn.Module, groups: Sequence[Sequence[str]] = DEFAULT_GROUPS, pdl: bool = False,
@@ -228,6 +261,16 @@ def set_lists_prefill(model: nn.Module, enabled: bool = True) -> int:
     layers = [l for l in layers if isinstance(l, VQuantLinear)]
     for l in layers:
         l.set_lists_prefill(enabled)
+    return len(layers)
+
+
+def set_list_decode(model: nn.Module, enabled: bool = True) -> int:
+    """`VQuantLinear.set_list_decode(enabled)` on every VQuantLinear of `model`, fused members included (it changes
+    only vector-length-16 layers the v = 16 list kernel takes).  Returns how many layers it reached."""
+    layers = [mod.layer if isinstance(mod, FusedMember) else mod for mod in model.modules()]
+    layers = [l for l in layers if isinstance(l, VQuantLinear)]
+    for l in layers:
+        l.set_list_decode(enabled)
     return len(layers)
 
 

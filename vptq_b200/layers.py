@@ -165,6 +165,7 @@ class VQuantLinear(nn.Module):
         self._quant_grad = False         # set_quant_grad
         self._batched_decode = False     # set_batched_decode
         self._lists_prefill = False      # set_lists_prefill
+        self._list_decode = False        # set_list_decode
 
     # ------------------------------------------------------------------------------------------
     def _tensors(self):
@@ -245,6 +246,26 @@ class VQuantLinear(nn.Module):
         full module's results bit for bit.  On a module that still has its packed words nothing changes.  Weight
         gradients (`set_quant_grad`) and saving the state_dict stay refused on a decode-only module."""
         self._lists_prefill = bool(enabled)
+        return self
+
+    def set_list_decode(self, enabled: bool = True) -> "VQuantLinear":
+        """Opt in to decode from index lists for a vector-length-16 layer (the v16-k65536 checkpoints): the
+        descriptor also carries lists with index rows of 16 outputs (4.25 bytes per index on top of the packed
+        words), and calls of 1..max tokens (4, 2 or 1: `native.lists16_max_tokens`) run the v = 16 list kernel
+        (include/vptq_b200_lists16.h), which stages each 4096-entry codebook slice in shared memory instead of
+        gathering the codebook through L1/L2.  Larger calls are routed as without the opt-in.  Its results may differ
+        from the default routes in the low-order bits; each token's outputs do not depend on the other tokens of the
+        call.  Backward is unchanged (the packed words are kept; `prepare(drop_packed=True)` stays refused).
+
+        Only eligible layers change: vector_len 16, one codebook group, no outlier columns, K = 4096 * (2..16),
+        Kr <= 256 and slices x column tiles <= the SM count.  On every other layer (v = 8 included) this does
+        nothing.  Turning it on drops a descriptor built without the lists (the next call or `prepare()` builds them):
+        call it before capturing CUDA graphs."""
+        enabled = bool(enabled)
+        if enabled and not self._list_decode and self.vector_len == 16 and self._desc_cache and \
+                not self._desc_cache[0].lists_stream:
+            self._desc_cache, self._desc_key = [], None
+        self._list_decode = enabled
         return self
 
     def _decode_only(self) -> bool:
@@ -356,7 +377,8 @@ class VQuantLinear(nn.Module):
             vector_quant_dim=self.vector_quant_dim, _desc_cache=self._desc_cache,
             _drop_packed=getattr(self, "_drop_request", False), _quant_grad=getattr(self, "_quant_grad", False),
             _batched_decode=getattr(self, "_batched_decode", False),
-            _lists_prefill=getattr(self, "_lists_prefill", False))
+            _lists_prefill=getattr(self, "_lists_prefill", False),
+            _list_decode=getattr(self, "_list_decode", False))
 
     def dequant(self) -> torch.Tensor:
         """Dense [out_features, in_features] weight through the CUDA dequant kernel (from the index lists on a

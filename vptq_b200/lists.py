@@ -23,6 +23,9 @@ A sum does not care about the order of its terms, so the fields of every index r
   * lists are padded to whole steps of 32 entries (every list has >= 1 step); the padding words are 0 and
     the kernel masks them with the list's tail count, so no null column is needed.
 
+Vector-length-16 layers (opt-in: VQuantLinear.set_list_decode, consumer csrc/gemv_lists16.cu) use the same format
+with index rows of 16 outputs (Ro = ceil(O / 16)).
+
 Storage: `stream` int32 [T][32] (step-major, units in increasing u), `tab` int32 [U + 1] with
 tab[u] = first step of unit u | (valid entries in the unit's LAST step) << 26, tab[U] = T.
 
@@ -54,10 +57,12 @@ def geometry(in_features: int, num_centroids: int) -> Tuple[int, int, int]:
 
 
 def eligible(*, vector_len: int, num_centroids: int, num_res_centroids: int, num_codebooks: int,
-             outlier_size: int, in_features: int) -> bool:
-    """Mirror of gemv_lists_eligible() (csrc/gemv_lists.cu) for the shape-only conditions."""
+             outlier_size: int, in_features: int, list_vector_len: int = 8) -> bool:
+    """Mirror of gemv_lists_eligible() (csrc/gemv_lists.cu) for the shape-only conditions.  list_vector_len=16 asks
+    about the lists of vector-length-16 layers instead (gemv_lists16_eligible, csrc/gemv_lists16.cu: the same K / Kr
+    rule)."""
     K = int(num_centroids)
-    return (vector_len == 8 and num_codebooks == 1 and outlier_size <= 0 and K >= 2 * SLICE_ENTRIES
+    return (list_vector_len in (8, 16) and vector_len == list_vector_len and num_codebooks == 1 and outlier_size <= 0 and K >= 2 * SLICE_ENTRIES
             and K % SLICE_ENTRIES == 0 and K // SLICE_ENTRIES <= 16 and num_res_centroids <= 256
             and 8 <= in_features <= 65535)
 
@@ -88,13 +93,16 @@ def deal_lists(stream: torch.Tensor, tab: torch.Tensor, threads: int = 0) -> tor
 
 
 def build_lists(indices: torch.Tensor, *, num_centroids: int, num_res_centroids: int, in_features: int,
-                out_features: int, perm: Optional[torch.Tensor], deal: Optional[bool] = None
+                out_features: int, perm: Optional[torch.Tensor], deal: Optional[bool] = None, vector_len: int = 8
                 ) -> Tuple[torch.Tensor, torch.Tensor, int]:
     """packed int32 [1, >=Ro, W] (+ perm [I], uint16 payload) -> (stream int32 [T, 32], tab int32 [U+1], TCW).
 
+    vector_len: outputs per index row, 8 or 16 (Ro = ceil(out_features / vector_len)); nothing else depends on it.
     deal: run `deal_lists` on the result (None = VPTQ_B200_LISTS_DEAL, default on)."""
     K, Kr, I = int(num_centroids), int(num_res_centroids), int(in_features)
-    Ro = (int(out_features) + 7) // 8
+    if vector_len not in (8, 16):
+        raise ValueError(f"index lists exist for vector_len 8 and 16, not {vector_len}")
+    Ro = (int(out_features) + vector_len - 1) // vector_len
     ib = K.bit_length() - 1
     rb = (Kr.bit_length() - 1) if Kr > 0 else 0
     NS, NT, TCW = geometry(I, K)
@@ -155,11 +163,11 @@ def build_lists(indices: torch.Tensor, *, num_centroids: int, num_res_centroids:
 
 def emulate(stream: torch.Tensor, tab: torch.Tensor, *, num_centroids: int, num_res_centroids: int,
             in_features: int, out_features: int, centroids: torch.Tensor, res_centroids: Optional[torch.Tensor],
-            xs: torch.Tensor) -> torch.Tensor:
+            xs: torch.Tensor, vector_len: int = 8) -> torch.Tensor:
     """float64 evaluation of sum_f xs[f] * (C[idx] + R[ridx]) straight from the lists, xs = x * scale in
-    ORIGINAL feature order (test aid: validates the format without a GPU).  Returns [Ro * 8]."""
-    K, Kr, I = int(num_centroids), int(num_res_centroids), int(in_features)
-    Ro = (int(out_features) + 7) // 8
+    ORIGINAL feature order (test aid: validates the format without a GPU).  Returns [Ro * vector_len]."""
+    K, Kr, I, v = int(num_centroids), int(num_res_centroids), int(in_features), int(vector_len)
+    Ro = (int(out_features) + v - 1) // v
     NS, NT, TCW = geometry(I, K)
     U = NS * NT * Ro
     T = stream.shape[0]
@@ -176,11 +184,11 @@ def emulate(stream: torch.Tensor, tab: torch.Tensor, *, num_centroids: int, num_
     f = t_of[:, None] * TCW + col
     f = torch.where(valid, f, torch.zeros_like(f))
     assert bool((f < I).all())
-    wt = centroids.reshape(K, 8).double()[s_of[:, None] * SLICE_ENTRIES + low]                  # [T, 32, 8]
+    wt = centroids.reshape(K, v).double()[s_of[:, None] * SLICE_ENTRIES + low]                  # [T, 32, v]
     if Kr > 0:
-        wt = wt + res_centroids.reshape(Kr, 8).double()[rix]
+        wt = wt + res_centroids.reshape(Kr, v).double()[rix]
     xv = torch.where(valid, xs.double().reshape(-1)[f], torch.zeros(1, dtype=torch.float64))
-    contrib = (wt * xv[:, :, None]).sum(1)                                                      # [T, 8]
-    y = torch.zeros(Ro, 8, dtype=torch.float64)
+    contrib = (wt * xv[:, :, None]).sum(1)                                                      # [T, v]
+    y = torch.zeros(Ro, v, dtype=torch.float64)
     y.index_add_(0, r_of, contrib)
     return y.reshape(-1)

@@ -52,6 +52,12 @@ LISTS_DENSE_EXPORTS = ("vptq_b200_lists_dense_version", "vptq_b200_lists_dense_w
                        "vptq_b200_lists_dequant", "vptq_b200_lists_quant_gemm")
 LISTS_DENSE_VERSION = 1
 
+# decode from the index lists of vector-length-16 layers (include/vptq_b200_lists16.h), same library
+LISTS16_EXPORTS = ("vptq_b200_lists16_version", "vptq_b200_quant_gemv_lists16_max_tokens",
+                   "vptq_b200_quant_gemv_lists16", "vptq_b200_lists16_build_host")
+LISTS16_VERSION = 1
+LISTS16_WORKSPACE_BYTES = 65536 * 4 + 65536 * 64
+
 MAX_FUSED, MAX_RANKS = 4, 8
 
 
@@ -192,6 +198,20 @@ def lib() -> ctypes.CDLL:
         if L.vptq_b200_lists_dense_version() != LISTS_DENSE_VERSION:
             raise RuntimeError(f"libvptq_b200.so lists-dense interface {L.vptq_b200_lists_dense_version()} != expected "
                                f"{LISTS_DENSE_VERSION}")
+        for f in LISTS16_EXPORTS:
+            if not hasattr(L, f):
+                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_lists16.h): rebuild it")
+        L.vptq_b200_lists16_version.restype = ctypes.c_int
+        L.vptq_b200_quant_gemv_lists16_max_tokens.argtypes = [i32, ctypes.POINTER(dp)]
+        L.vptq_b200_quant_gemv_lists16_max_tokens.restype = ctypes.c_int
+        L.vptq_b200_quant_gemv_lists16.argtypes = [i32, ctypes.POINTER(dp), vp, i64, ctypes.POINTER(vp),
+                                                   ctypes.POINTER(i64), i32, vp, sz, u32, vp]
+        L.vptq_b200_quant_gemv_lists16.restype = ctypes.c_int
+        L.vptq_b200_lists16_build_host.argtypes = L.vptq_b200_lists_build_host.argtypes
+        L.vptq_b200_lists16_build_host.restype = ctypes.c_int
+        if L.vptq_b200_lists16_version() != LISTS16_VERSION:
+            raise RuntimeError(f"libvptq_b200.so lists16 interface {L.vptq_b200_lists16_version()} != expected "
+                               f"{LISTS16_VERSION}")
         _lib = L
     return _lib
 
@@ -244,7 +264,8 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
               outlier_indices: Optional[torch.Tensor], outlier_centroids: Optional[torch.Tensor],
               perm: Optional[torch.Tensor], weight_scale: Optional[torch.Tensor],
               weight_bias: Optional[torch.Tensor], bias: Optional[torch.Tensor],
-              derive: bool = True, lists: Optional[bool] = None, drop_packed: bool = False) -> LinearDesc:
+              derive: bool = True, lists: Optional[bool] = None, drop_packed: bool = False,
+              lists16: bool = False) -> LinearDesc:
     """Describe one layer's tensors for the C ABI.  Tensors are borrowed: keep them alive.
 
     With `derive` (default) the load-time derivatives the ABI accepts are built here, once:
@@ -255,6 +276,10 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
     large-codebook layers gather from shared memory; costs 4 bytes per index (+ ~6 % padding) on top
     of the packed words (3 bytes per index for the 65536+256 configuration).  None = the
     VPTQ_B200_LISTS environment variable (default on); ignored for layers the list kernel does not cover.
+
+    `lists16`: build the index lists of a vector-length-16 layer (index rows of 16 outputs) for
+    include/vptq_b200_lists16.h: 4.25 bytes per index on top of the packed words.  Opt-in only
+    (VQuantLinear.set_list_decode); ignored for layers that kernel does not cover.
 
     `drop_packed`: decode-only descriptor -- once the lists are built the descriptor forgets the packed words
     (`indices` = NULL), so the caller may free them: 4.2 instead of 7.2 bytes per index.  Multi-token calls,
@@ -312,7 +337,21 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
                                               out_features=d.out_features, perm=perm)
         d.lists_stream, d.lists_tab, d.lists_tile_cols = stream.data_ptr(), tab.data_ptr(), int(tcw)
         d._keep = d._keep + (stream, tab)
+    if lists16 and derive and d.vector_len == 16 and _lists.eligible(
+            vector_len=d.vector_len, num_centroids=d.num_centroids, num_res_centroids=d.num_res_centroids,
+            num_codebooks=d.num_codebooks, outlier_size=d.outlier_size, in_features=d.in_features,
+            list_vector_len=16) and (
+            weight_scale is None or (weight_scale.data_ptr() % 16 == 0 and weight_bias.data_ptr() % 16 == 0)) and (
+            _lists.launchable(d.in_features, d.num_centroids, _sm_count(indices.device))):
+        stream, tab, tcw = _lists.build_lists(indices, num_centroids=d.num_centroids,
+                                              num_res_centroids=d.num_res_centroids, in_features=d.in_features,
+                                              out_features=d.out_features, perm=perm, vector_len=16)
+        d.lists_stream, d.lists_tab, d.lists_tile_cols = stream.data_ptr(), tab.data_ptr(), int(tcw)
+        d._keep = d._keep + (stream, tab)
     if drop_packed:
+        if d.vector_len != 8 and d.lists_stream:
+            raise RuntimeError("drop_packed: decode-only descriptors exist for vector_len 8 only (a vector-length-16 "
+                               "layer's lists serve single- and few-token decode, not prefill or dequant)")
         if not d.lists_stream:
             raise RuntimeError("drop_packed: this layer has no index lists (not eligible, its slices x column tiles "
                                "exceed the device's SM count, or lists=False)")
@@ -521,6 +560,51 @@ class FusedGemvBatch:
                                                   self.stride_arr, x2d.shape[0], ws.data_ptr(), ws.numel(), flags,
                                                   _stream(dev))
         check(rc, "vptq_b200_quant_gemv_batch")
+
+
+def lists16_max_tokens(descs) -> int:
+    """vptq_b200_quant_gemv_lists16_max_tokens: the largest token count (4, 2 or 1) the vector-length-16 list kernel
+    takes for these layers (one descriptor or a list of 1..MAX_FUSED reading the same x) on the current device, 0 when
+    they are not eligible.  Cached on the first descriptor (the answer depends on the shapes and the device only)."""
+    descs = [descs] if isinstance(descs, LinearDesc) else list(descs)
+    if not descs or not all(d.lists_stream and d.vector_len == 16 for d in descs):
+        return 0
+    idx = torch.cuda.current_device()
+    cache = descs[0].__dict__.setdefault("_lists16_max", {})
+    key = (idx,) + tuple(id(d) for d in descs)
+    v = cache.get(key)
+    if v is None:
+        v = cache[key] = int(lib().vptq_b200_quant_gemv_lists16_max_tokens(len(descs), _desc_array(descs)))
+    return v
+
+
+def quant_gemv_lists16(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, flags: int = 0) -> None:
+    """y2d [tokens, O] = x2d [tokens, I] @ W^T + bias by the vector-length-16 list kernel
+    (vptq_b200_quant_gemv_lists16), 1 <= tokens <= lists16_max_tokens(desc)."""
+    FusedGemvLists16([desc], [y2d])(x2d, flags)
+
+
+class FusedGemvLists16:
+    """Prepared argument arrays for vptq_b200_quant_gemv_lists16 (1..MAX_FUSED vector-length-16 layers sharing one
+    input, 1..4 tokens).  No fall-back: a refusal raises."""
+
+    def __init__(self, descs, ys):
+        n = len(descs)
+        if not 1 <= n <= MAX_FUSED or len(ys) != n:
+            raise RuntimeError(f"FusedGemvLists16 takes 1..{MAX_FUSED} layers with one output each")
+        self.n, self.descs, self.ys = n, list(descs), list(ys)
+        self.desc_arr = _desc_array(self.descs)
+        self.y_arr = (ctypes.c_void_p * n)(*[y.data_ptr() for y in ys])
+        self.stride_arr = (ctypes.c_int64 * n)(*[row_pitch(y) for y in ys])
+
+    def __call__(self, x2d: torch.Tensor, flags: int = 0) -> None:
+        dev = x2d.device
+        with _on_device(dev):
+            ws = workspace(dev, LISTS16_WORKSPACE_BYTES)
+            rc = lib().vptq_b200_quant_gemv_lists16(self.n, self.desc_arr, x2d.data_ptr(), row_pitch(x2d), self.y_arr,
+                                                    self.stride_arr, x2d.shape[0], ws.data_ptr(), ws.numel(), flags,
+                                                    _stream(dev))
+        check(rc, "vptq_b200_quant_gemv_lists16")
 
 
 class FusedGemvTP:

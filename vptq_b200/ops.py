@@ -11,7 +11,8 @@ Function names, argument order and argument meaning are the reference's
   VQuantLinear.set_batched_decode): 2..8 tokens of a layer with index lists -> the batched list kernel.  Opt-in
   (`_lists_prefill`, VQuantLinear.set_lists_prefill): a decode-only descriptor takes every call the list kernels do
   not through the GEMM with the weight written from the index lists (include/vptq_b200_lists_dense.h), and its input
-  gradient likewise;
+  gradient likewise.  Opt-in (`_list_decode`, VQuantLinear.set_list_decode): 1..lists16_max_tokens tokens of a
+  vector-length-16 layer with index lists -> the v = 16 list kernel (include/vptq_b200_lists16.h);
 * `argsort(perm)` is not recomputed on every call (the reference does, :208-211).
 """
 from __future__ import annotations
@@ -29,7 +30,7 @@ __all__ = ["dequant", "quant_gemm", "quant_gemv_v2"]
 def _desc(*, dtype, indices, centroids, outlier_indices, outlier_centroids, residual_centroids, perm,
           weight_scale, weight_bias, bias, vector_len, outlier_vector_len, num_codebooks, num_centroids,
           num_outlier_centroids, num_res_centroids, group_size, outlier_size, in_features, out_features,
-          derive=True, lists=None, drop_packed=False):
+          derive=True, lists=None, drop_packed=False, lists16=False):
     if perm is not None and perm.dtype not in (torch.int16, torch.uint16):
         # unpacked checkpoints keep perm as int64 (vqlinear.py:191-196)
         perm = perm.to(torch.int64).to(torch.uint16).contiguous()
@@ -40,7 +41,7 @@ def _desc(*, dtype, indices, centroids, outlier_indices, outlier_centroids, resi
         outlier_vector_len=outlier_vector_len, num_outlier_centroids=num_outlier_centroids, indices=indices,
         centroids=centroids, res_centroids=residual_centroids, outlier_indices=outlier_indices,
         outlier_centroids=outlier_centroids, perm=perm, weight_scale=weight_scale, weight_bias=weight_bias,
-        bias=bias, derive=derive, lists=lists, drop_packed=drop_packed), perm
+        bias=bias, derive=derive, lists=lists, drop_packed=drop_packed, lists16=lists16), perm
 
 
 def dequant(
@@ -179,6 +180,7 @@ def quant_gemm(
     _quant_grad: bool = False,
     _batched_decode: bool = False,
     _lists_prefill: bool = False,
+    _list_decode: bool = False,
 ) -> torch.Tensor:
     """y = x @ W^T + bias for one VPTQ layer (reference: vptq/ops/quant_gemm.py:161-275).
 
@@ -190,7 +192,11 @@ def quant_gemm(
 
     `_lists_prefill` (VQuantLinear.set_lists_prefill): on a decode-only descriptor, calls neither list kernel takes
     and the input gradient run the GEMM with the weight written from the index lists; no effect on a descriptor
-    that still has its packed words."""
+    that still has its packed words.
+
+    `_list_decode` (VQuantLinear.set_list_decode): a kept descriptor of a vector-length-16 layer carries index lists,
+    and 1..lists16_max_tokens tokens run the v = 16 list kernel (include/vptq_b200_lists16.h); every other call is
+    routed as without it."""
     if vector_quant_dim == "in":
         raise ValueError("Not implemented yet.")
     if not is_indice_packed:
@@ -214,7 +220,8 @@ def quant_gemm(
             group_size=group_size, outlier_size=outlier_size, in_features=in_features, out_features=out_features,
             # a one-off descriptor (reference-style direct call) must not pay for re-bucketing the whole layer:
             # the slice x tile lists are built only when the caller keeps the descriptor (VQuantLinear does)
-            lists=None if _desc_cache is not None else False, drop_packed=_drop_packed)
+            lists=None if _desc_cache is not None else False, drop_packed=_drop_packed,
+            lists16=_list_decode and _desc_cache is not None)
         if _desc_cache is not None:
             _desc_cache.extend([desc, perm_])   # keep the converted perm alive with the descriptor
     x2d = x.reshape(-1, in_features)
@@ -231,23 +238,27 @@ def quant_gemm(
             if not quant:
                 layer = (indices, centroids, residual_centroids, outlier_indices, outlier_centroids, perm,
                          weight_scale, weight_bias)
-                y = _QuantLinearFn.apply(x2d, bias, keep, out_features, (_batched_decode, _lists_prefill),
+                y = _QuantLinearFn.apply(x2d, bias, keep, out_features, (_batched_decode, _lists_prefill, _list_decode),
                                          *[t for t in layer if t is not None])
             else:
                 others = [t for t in (indices, outlier_indices, perm) if t is not None]
-                y = _QuantLinearWgradFn.apply(x2d, bias, keep, out_features, (_batched_decode, _lists_prefill),
+                y = _QuantLinearWgradFn.apply(x2d, bias, keep, out_features, (_batched_decode, _lists_prefill, _list_decode),
                                               tuple(n for n, _ in slots), *[t for _, t in slots], *others)
             return y.reshape(*x.shape[:-1], out_features)
-    return _forward(desc, x2d, out_features, _batched_decode, _lists_prefill).reshape(*x.shape[:-1], out_features)
+    return _forward(desc, x2d, out_features, _batched_decode, _lists_prefill, _list_decode).reshape(
+        *x.shape[:-1], out_features)
 
 
 def _forward(desc, x2d: torch.Tensor, out_features: int, batched: bool = False,
-             lists_prefill: bool = False) -> torch.Tensor:
+             lists_prefill: bool = False, list_decode: bool = False) -> torch.Tensor:
     tokens = x2d.shape[0]
     y = torch.empty(tokens, out_features, dtype=x2d.dtype, device=x2d.device)
     if tokens == 0:
         return y
-    if batched and tokens >= 2 and desc.lists_stream and x2d.data_ptr() % 16 == 0 and \
+    if list_decode and desc.vector_len == 16 and desc.lists_stream and x2d.data_ptr() % 16 == 0 and \
+            tokens <= native.lists16_max_tokens(desc):
+        native.quant_gemv_lists16(desc, x2d, y)
+    elif batched and tokens >= 2 and desc.lists_stream and x2d.data_ptr() % 16 == 0 and \
             tokens <= native.batch_max_tokens(desc):
         native.quant_gemv_batch(desc, x2d, y)
     elif lists_prefill and tokens >= 2 and not desc.indices:
