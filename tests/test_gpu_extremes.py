@@ -661,3 +661,194 @@ def test_batch_graph_replay_poisoned_then_clean():
         torch.cuda.synchronize()
         assert torch.equal(y, clean), vname
     _batch.head_zero()
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# the vector-length-16 list kernel (1..4 tokens per launch; its class records are always on)
+# ------------------------------------------------------------------------------------------------------------------
+def _v16_const_layer(value, dtype="fp16"):
+    """v = 16, K = 8192 (NS = 2, Q = 2: unit sums are admitted below 2^33 / 2 = 2^32), no perm / norm, every main
+    entry `value`"""
+    L = vo.make_layer(in_features=1024, out_features=264, vector_len=16, num_centroids=8192, enable_perm=False,
+                      enable_norm=False, seed=15, dtype=dtype)
+    L.centroids = encode(np.full(L.centroids.shape, value), L.dtype)
+    return L
+
+
+def _v16(L, x, ys=None):
+    from _lists16 import only_kernel, run
+    d = _lists16_desc(L)
+    y = run(d, x) if ys is None else ys
+    only_kernel(lambda: run(d, x, [y]), launches=1)
+    torch.cuda.synchronize()
+    return y
+
+
+def _lists16_desc(L):
+    from _lists16 import desc_of
+    key = id(L)
+    if key not in _V16:
+        _V16.clear()
+        _V16[key] = (L, desc_of(L))
+    return _V16[key][1]
+
+
+_V16 = {}
+
+
+@pytest.mark.parametrize("second_unit", [False, True])
+def test_v16_fp16_past_the_fixed_point_range_one_token_of_four(second_unit):
+    """token 2 of 4 hits entries of 60000 with x = 60000: alone, one slice-0 unit of three such terms (1.08e10, past
+    2^33); with `second_unit`, two units (slices 0 and 1) of two terms each (7.2e9 each: inside 2^33, past
+    2^33 / 2^ceil(log2 Q) = 2^32, and their 2^-30 fixed-point sum past 2^63).  +inf or NaN, never -inf or finite;
+    the other three tokens bit-identical to a launch in which token 2 is small too"""
+    L = _v16_const_layer(60000.0)
+    idx = L.meta["idx"]
+    split = 2 if second_unit else 3
+    idx[0, :, :split] = idx[0, :, :split] % 4096                      # slice 0
+    idx[0, :, split:4] = 4096 + idx[0, :, split:4] % 4096             # slice 1
+    L.indices = vo.pack_index(idx, L.index_bits)
+    W = torch.from_numpy(dense64(L)).cuda()
+    x = (_sweep_x(4, 1024, "fp16", seed=13) * 2.0 ** -10).half()
+    clean = _v16(L, x).clone()
+    assert torch.isfinite(clean).all()
+    xb = x.clone()
+    xb[2, :4 if second_unit else 3] = 60000.0
+    assert bool((y_star(L, xb[2:3], W) > 1e10).all())
+    y = _v16(L, xb)
+    assert bool(((y[2] == float("inf")) | torch.isnan(y[2])).all()), y[2]
+    others = [0, 1, 3]
+    assert torch.equal(y[others], clean[others])
+    assert torch.equal(_v16(L, x), clean)                              # (the records were cleared)
+    _batch.head_zero()
+
+
+@pytest.mark.parametrize("sign", [1, -1])
+def test_v16_fp16_output_overflow(sign):
+    """every unit sum well inside the fixed point, y = sign * 71680 > 65504: +-inf at every token count"""
+    L = _v16_const_layer(1.0)
+    x = torch.full((4, 1024), 70.0 * sign, dtype=torch.float16, device="cuda")
+    assert float(y_star(L, x[:1]).min()) * sign > 65520
+    for tokens in (1, 2, 3, 4):
+        y = _v16(L, x[:tokens].clone())
+        assert bool((y == sign * float("inf")).all()), tokens
+    _batch.head_zero()
+
+
+def test_v16_bf16_outputs_beyond_the_fixed_point_range():
+    """one main entry element of 2^36, used once in index rows 1 and 7 with x = 1 there: outputs of ~2^36 >= 2^33 in
+    all four tokens.  NaN or correct there, correct everywhere else"""
+    L = vo.make_layer(in_features=1024, out_features=264, vector_len=16, num_centroids=65536, num_res_centroids=256,
+                      dtype="bf16", bias=True, llm_like=False, seed=6)
+    L = isolate(L, main={K_ARB: [1, 7]})
+    e = 3
+    L = inject(L, "C", 2.0 ** 36, k=K_ARB, e=e)
+    x = torch.from_numpy(vo.to_f32(vo.make_x(4, 1024, "bf16", seed=3), "bf16")).cuda().to(torch.bfloat16)
+    for r in (1, 7):
+        f = feature_of(L, isolated_column(L, r, K_ARB))
+        x[:, f] = 1.0
+        s = vo.to_f32(L.weight_scale, "bf16")
+        s[f] = 1.0
+        L.weight_scale = encode(s, "bf16")
+    ys = y_star(L, x)
+    hit = torch.zeros(L.out_features, dtype=torch.bool, device="cuda")
+    hit[[16 + e, 112 + e]] = True
+    assert bool((ys[:, hit].abs() >= 2.0 ** 33).all()) and bool((ys[:, ~hit].abs() < 1e3).all())
+    y = _v16(L, x).double()
+    rest = float((y[:, ~hit] - ys[:, ~hit]).abs().max() / ys[:, ~hit].abs().max())
+    assert rest <= TOL["bf16"], rest
+    ok = ((y[:, hit] - ys[:, hit]).abs() / ys[:, hit].abs() <= TOL["bf16"]) | torch.isnan(y[:, hit])
+    assert bool(ok.all()), y[:, hit]
+    _batch.head_zero()
+
+
+def _v16_sweep_layer(dtype):
+    L = vo.make_layer(in_features=1004, out_features=264, vector_len=16, num_centroids=65536, num_res_centroids=256,
+                      dtype=dtype, seed=8)
+    s = 1.0 + np.abs(0.1 * np.random.default_rng(1).standard_normal(1004))
+    L.weight_scale = encode(np.minimum(s, 1.9), dtype)
+    return L
+
+
+@pytest.mark.parametrize("dtype,ks", [("fp16", (-8, -2, 3, 8)), ("bf16", (-24, -9, 0, 8))], ids=["fp16", "bf16"])
+def test_v16_magnitude_spread(dtype, ks):
+    """one 4-token launch whose tokens are scaled by 2^k, k spread over the range: each token within its own bar (the
+    kernel's arithmetic in fp64; twice that against the exact product) and the same bits as that token alone"""
+    L = _v16_sweep_layer(dtype)
+    q = _batch.q_of(1004, 65536)
+    x = _sweep_x(4, 1004, dtype, seed=14) * torch.tensor([2.0 ** k for k in ks], device="cuda")[:, None]
+    x = x.to(_dt(L))
+    y = _v16(L, x)
+    kstar, ys = _batch.kernel_star(L, x), y_star(L, x)
+    for t in range(4):
+        _batch.assert_close(y[t:t + 1], kstar[t:t + 1], dtype, q)
+        _batch.assert_close(y[t:t + 1], ys[t:t + 1], dtype, q, factor=2.0)
+        assert torch.equal(_v16(L, x[t:t + 1].clone()), y[t:t + 1]), t
+    _batch.head_zero()
+
+
+@pytest.mark.parametrize("dtype,ks", [("fp16", range(-8, 9)), ("bf16", range(-24, 9, 2))], ids=["fp16", "bf16"])
+def test_v16_scaling_within_the_documented_floor(dtype, ks):
+    """|y - y*| <= TOL max|y*| + Q 2^-31 at every scale, 1 and 3 tokens (bf16 down to outputs around 2^-25)"""
+    L = _v16_sweep_layer(dtype)
+    Q = _batch.q_of(1004, 65536)
+    x = _sweep_x(3, 1004, dtype, seed=12)
+    W = torch.from_numpy(dense64(L)).cuda()
+    smallest = float("inf")
+    for k in ks:
+        xk = x * 2.0 ** k
+        for tokens in (1, 3):
+            y = _v16(L, xk[:tokens].clone()).double()
+            ys = y_star(L, xk[:tokens], W)
+            bound = TOL[dtype] * float(ys.abs().max()) + Q * 2.0 ** -31
+            err = float((y - ys).abs().max())
+            smallest = min(smallest, float(ys.abs().max()))
+            assert err <= bound, (k, tokens, err, bound)
+    if dtype == "bf16":
+        assert smallest < 2.0 ** -22            # the sweep reached outputs where only the floor holds
+    _batch.head_zero()
+
+
+def test_v16_graph_replay_clean_poisoned_clean():
+    """CUDA graph of one 4-token v = 16 launch, replayed with clean, poisoned (NaN, +inf, -inf in one feature of
+    token 3) and clean x: the poisoned token's classes those of the kernel's arithmetic in fp64, the other tokens and
+    every clean replay the bits of the first clean replay"""
+    from _lists16 import run
+    from vptq_b200 import native
+    L = vo.make_layer(in_features=1004, out_features=264, vector_len=16, num_centroids=65536, num_res_centroids=256,
+                      seed=17, bias=True)
+    d = _lists16_desc(L)
+    x0 = torch.from_numpy(vo.to_f32(vo.make_x(4, 1004, "fp16", seed=3), "fp16")).cuda().half()
+    xbuf = torch.zeros(4, 1008, dtype=torch.float16, device="cuda")[:, :1004]
+    xbuf.copy_(x0)
+    y = torch.empty(4, 264, dtype=torch.float16, device="cuda")
+    fb = native.FusedGemvLists16([d], [y])
+    eager = run(d, x0.clone()).clone()
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        fb(xbuf, native.FLAG_PDL)
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, stream=s):
+            fb(xbuf, native.FLAG_PDL)
+    y.fill_(0)
+    g.replay()
+    torch.cuda.synchronize()
+    clean = y.clone()
+    assert torch.equal(clean, eager)
+    for vname, v in VALUES.items():
+        xi = x0.clone()
+        xi[3, 10] = v
+        xbuf.copy_(xi)
+        y.fill_(0)
+        g.replay()
+        torch.cuda.synchronize()
+        assert torch.equal(y[:3], clean[:3]), vname
+        assert torch.equal(classify(y[3]), classify(_batch.kernel_star(L, xi)[3])), vname
+        assert not torch.isfinite(y[3]).any(), vname
+        xbuf.copy_(x0)
+        y.fill_(0)
+        g.replay()
+        torch.cuda.synchronize()
+        assert torch.equal(y, clean), vname
+    _batch.head_zero()

@@ -42,6 +42,18 @@ CONFIGS = {
     "v": dict(in_features=1024, out_features=136, num_centroids=65536, num_res_centroids=256, bias=True, seed=13),
     "other": dict(in_features=1024, out_features=264, num_centroids=65536, num_res_centroids=256, bias=True, seed=99),
     "other_q": dict(in_features=1024, out_features=264, num_centroids=65536, num_res_centroids=256, seed=98),
+    # vector-length-16 layers (the v = 16 list kernel)
+    "v16": dict(in_features=1024, out_features=264, vector_len=16, num_centroids=65536, num_res_centroids=256, bias=True),
+    "v16_bf16": dict(in_features=1024, out_features=264, vector_len=16, num_centroids=65536, num_res_centroids=256,
+                     bias=True, dtype="bf16"),
+    "v16_other": dict(in_features=1024, out_features=264, vector_len=16, num_centroids=65536, num_res_centroids=256,
+                      bias=True, seed=97),
+    "v16_q": dict(in_features=1024, out_features=264, vector_len=16, num_centroids=65536, num_res_centroids=256, seed=21),
+    "v16_k": dict(in_features=1024, out_features=128, vector_len=16, num_centroids=65536, num_res_centroids=256, seed=22),
+    "v16_v": dict(in_features=1024, out_features=136, vector_len=16, num_centroids=65536, num_res_centroids=256,
+                  bias=True, seed=23),
+    "v16_other_q": dict(in_features=1024, out_features=264, vector_len=16, num_centroids=65536, num_res_centroids=256,
+                        seed=96),
 }
 _LAYERS = {}
 
@@ -63,6 +75,8 @@ KERNELS = {
     "direct": lambda n: ran(n, "dequant_o8_kernel") and ran(n, "gemm_tn_wgmma") and not ran(n, "prefill_prep_x"),
     "prep": lambda n: ran(n, "prefill_prep_x") and ran(n, "gemm_tn_wgmma") and not ran(n, "dequant_o8_kernel"),
     "batch": lambda n: sum(ran([k], "gemv_lists_batch_kernel") for k in n) == 1 and not ran(n, "gemv_lists_kernel")
+    and not ran(n, "gemv_kernel") and not ran(n, "gemm_tn_wgmma"),
+    "lists16": lambda n: sum(ran([k], "gemv_lists16_kernel") for k in n) == 1 and not ran(n, "gemv_lists_kernel")
     and not ran(n, "gemv_kernel") and not ran(n, "gemm_tn_wgmma"),
 }
 
@@ -967,6 +981,304 @@ def test_batch_pdl_chain_of_a_llama_decoder_layer():
             assert same(o, r), (tokens, k)
         for k, st in enumerate(stages):
             src = x0 if k == 0 else [None, ref[0][:, :4096], ref[1], ref[2][:, :14336], ref[3]][k]
+            a = 0
+            for l in st:
+                rows = l.sample(16, seed=k)
+                Ls, cols, keep = l.oracle(rows)
+                idx = torch.from_numpy(np.nonzero(keep)[0]).cuda()
+                ys = ref[k][:, a:a + l.O][:, torch.from_numpy(cols[keep]).cuda()]
+                assert_close(ys, kernel_star(Ls, src)[:, idx], l.dtype, q_of(l.I, l.K))
+                a += l.O
+        del g
+    heads_at_rest()
+
+
+# ================================================================================================ vector-length-16 decode
+V16_QKV = ("v16_q", "v16_k", "v16_v")
+
+
+def listed16(L):
+    return make_module(L).set_list_decode(True)
+
+
+def fresh_qkv16(layers):
+    """a new fused v = 16 q/k/v group with the opt-in, holding copies of `layers`' tensors"""
+    from vptq_b200 import fuse, set_list_decode
+    f = QKV(V16_QKV)
+    for name, l in zip(("q_proj", "k_proj", "v_proj"), layers):
+        getattr(f, name).load_state_dict(l.state_dict())
+    fuse(f)
+    set_list_decode(f)
+    return f
+
+
+def qkv16_oracle_check(x, y, names=V16_QKV):
+    a = 0
+    for n in names:
+        L = layer(n)
+        close64(L, x, y[:, a:a + L.out_features])
+        a += L.out_features
+
+
+def test_v16_graphs_across_growth_capture_streams_and_a_second_stream():
+    """A1 + A2 + A6 for the v = 16 route: a graph captured on a side stream survives eager workspace growth; a graph
+    captured on torch's capture stream (a workspace private to the capture) replays last-captured first; a v = 16
+    stream and a single-token v = 8 list stream run at once"""
+    from vptq_b200 import native
+    L, Lp, L8 = layer("v16"), layer("prep"), layer("lists")
+    m, mp, m8 = listed16(L), make_module(Lp), make_module(L8)
+    x3, x4, x1 = xs(L, 3, seed=3), xs(L, 4, seed=4), xs(L8, 1, seed=1)
+    assert_route("lists16", lambda: m(x3))
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s), torch.no_grad():
+        e3, e4 = m(x3), m(x4)
+        g3 = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g3, stream=s):
+            y3 = m(x3)
+        old = weakref.ref(native._workspaces[ws_key(s)])
+        for t in (300, 8192):
+            x = xs(Lp, t, seed=t)
+            close64(Lp, x, mp(x))
+        assert native._workspaces[ws_key(s)] is not old()
+    assert old() is not None
+    torch.cuda.current_stream().wait_stream(s)
+    with torch.no_grad():
+        g4 = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g4):
+            y4 = m(x4)
+    assert ws_key(torch.cuda.graphs.graph.default_capture_stream) not in native._workspaces
+    with torch.no_grad():
+        for rep in range(3):
+            g4.replay()
+            with torch.cuda.stream(s):
+                g3.replay()
+            assert same(m(x3), e3)
+            torch.cuda.synchronize()
+            assert same(y4, e4) and same(y3, e3), rep
+        serial1 = m8(x1)
+        streams = [torch.cuda.Stream(), torch.cuda.Stream()]
+        for st in streams:
+            st.wait_stream(torch.cuda.current_stream())
+        outs = [[], []]
+        for _ in range(30):
+            with torch.cuda.stream(streams[0]):
+                outs[0].append(m(x4))
+            with torch.cuda.stream(streams[1]):
+                outs[1].append(m8(x1))
+    torch.cuda.synchronize()
+    assert all(same(y, e4) for y in outs[0]) and all(same(y, serial1) for y in outs[1])
+    fresh = listed16(L)
+    with torch.no_grad():
+        assert same(fresh(x3), e3) and same(fresh(x4), e4)
+    close64(L, x3, e3)
+    close64(L, x4, e4)
+    heads_at_rest()
+
+
+def test_v16_on_the_shared_workspace():
+    """A5: the v = 16 route interleaved on one stream's workspace with the v = 8 list, batched, generic, prefill,
+    dequant, dgrad and weight-gradient ops, each result the bits of the op alone"""
+    from vptq_b200 import native
+    ops = _ops()
+    L, L8 = layer("v16"), layer("lists")
+    m16, mb = listed16(L), make_module(L8).set_batched_decode(True)
+    x3, x5 = xs(L, 3, seed=33), xs(L8, 5, seed=55)
+    ops["lists16"] = lambda: m16(x3)
+    ops["batch"] = lambda: mb(x5)
+    alone = {}
+    for name, fn in ops.items():
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s), torch.no_grad():
+            alone[name] = fn()
+        s.synchronize()
+    with torch.no_grad():
+        assert_route("lists16", lambda: m16(x3))
+    close64(L, x3, alone["lists16"])
+    names = list(ops) + ["lists16"] * 4
+    random.Random(16).shuffle(names)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s), torch.no_grad():
+        for name in names:
+            y = ops[name]()
+            s.synchronize()
+            assert int(native._workspaces[ws_key(s)][:ZERO].count_nonzero()) == 0, name
+            assert same(y, alone[name]), name
+    heads_at_rest()
+
+
+def test_v16_graph_after_codebook_mul_without_prepare():
+    """B1: the v = 16 kernel reads the checkpoint's codebooks and original-order weight_scale / weight_bias directly,
+    so in-place updates of them need no refresh: mul_ of every float tensor, NO prepare(), replay -- the bits of a
+    fresh module with the opt-in"""
+    L = layer("v16")
+    m = listed16(L)
+    m.prepare()
+    x = xs(L, 4, seed=6)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s), torch.no_grad():
+        before = m(x).clone()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, stream=s):
+            y = m(x)
+    torch.cuda.current_stream().wait_stream(s)
+    with torch.no_grad():
+        for k, p in enumerate((m.centroids.weight, m.res_centroids.weight, m.weight_scale, m.weight_bias, m.bias)):
+            p.mul_(1.0 + 0.125 * (k + 1))
+    fresh = fresh_of(m, L).set_list_decode(True)
+    with torch.cuda.stream(s):
+        g.replay()
+    torch.cuda.synchronize()
+    with torch.no_grad():
+        assert not same(y, before)
+        assert_route("lists16", lambda: fresh(x))
+        assert same(y, fresh(x))
+        for t in (1, 2, 3):
+            xt = xs(L, t, seed=70 + t)
+            assert same(m(xt), fresh(xt)), t
+    close64(layer_of(m, L), x, y)
+    heads_at_rest()
+
+
+@pytest.mark.parametrize("change", ["copy_indices", "permute_perm"])
+def test_v16_eager_after_changes(change):
+    """B2 for the v = 16 route: the lists are rebuilt from the new indices / perm and the v = 16 kernel still runs"""
+    L, Lo = layer("v16"), layer("v16_other")
+    m, other = listed16(L), make_module(Lo)
+    with torch.no_grad():
+        m(xs(L, 3))
+        if change == "copy_indices":
+            m.indices.copy_(other.indices)
+        else:
+            p = torch.randperm(L.in_features, generator=torch.Generator().manual_seed(1)).cuda()
+            m.perm.copy_(m.perm[p])
+        fresh = fresh_of(m, L).set_list_decode(True)
+        for t in (1, 2, 4):
+            x = xs(L, t, seed=80 + t)
+            assert_route("lists16", lambda: m(x))
+            y = m(x)
+            assert same(y, fresh(x)), (change, t)
+            close64(layer_of(m, L), x, y)
+    heads_at_rest()
+
+
+def test_v16_load_state_dict_through_fuse():
+    import vptq_b200
+    p = QKV(V16_QKV)
+    vptq_b200.fuse(p)
+    vptq_b200.set_list_decode(p)
+    x3 = xs(layer("v16_q"), 3, seed=5)
+    with torch.no_grad():
+        p(x3)
+    sd = {**{"q_proj." + k: v for k, v in make_module(layer("v16_other_q")).state_dict().items()},
+          **{"k_proj." + k: v for k, v in p.k_proj.layer.state_dict().items()},
+          **{"v_proj." + k: v for k, v in p.v_proj.layer.state_dict().items()}}
+    p.load_state_dict(sd)
+    fresh = fresh_qkv16([make_module(layer("v16_other_q")), p.k_proj.layer, p.v_proj.layer])
+    with torch.no_grad():
+        y = p(x3)                                    # rebuilds q_proj's descriptor and lists
+        assert_route("lists16", lambda: p(x3))
+        assert same(y, fresh(x3))
+    close64(layer("v16_other_q"), x3, y[:, :264])
+    heads_at_rest()
+
+
+def test_v16_under_inference_mode():
+    """C1 / C2: a module and a fused group under torch.inference_mode(), a graph included, equal to no_grad"""
+    import vptq_b200
+    L = layer("v16_bf16")
+    m = listed16(L)
+    p = QKV(V16_QKV)
+    vptq_b200.fuse(p)
+    vptq_b200.set_list_decode(p)
+    x, xq = xs(L, 3, seed=7), xs(layer("v16_q"), 4, seed=4)
+    with torch.no_grad():
+        ref, refq = m(x), p(xq)
+    with torch.inference_mode():
+        xi, xqi = x.clone(), xq.clone()
+        assert_route("lists16", lambda: m(xi))
+        assert_route("lists16", lambda: p(xqi))
+        got, gotq = m(xi), p(xqi)
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            p(xqi)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=s):
+                yg = p(xqi)
+            g.replay()
+        torch.cuda.synchronize()
+    assert same(got, ref) and same(gotq, refq) and same(yg, refq)
+    fresh = fresh_qkv16([p.q_proj.layer, p.k_proj.layer, p.v_proj.layer])
+    with torch.no_grad():
+        assert same(fresh(xq), refq)
+    close64(L, x, got)
+    qkv16_oracle_check(xq, gotq)
+    heads_at_rest()
+
+
+def test_v16_pdl_chain_of_a_70b_decoder_layer():
+    """Llama-3-70B / Nemotron-70B decoder layer of v = 16 launches, each with programmatic dependent launch and reading
+    the previous launch's output view directly: q/k/v -> o (on the q slice) -> gate/up -> down (on the gate slice) ->
+    the next q/k/v.  Eager and as one CUDA graph, every stage the bits of the same launches run one at a time without
+    PDL, and within the bar on the x it consumed"""
+    from _batch import assert_close, kernel_star, q_of
+    from _lists16 import GpuLayer16
+    from vptq_b200 import native
+    qkv = [GpuLayer16(8192, o, seed=90 + k) for k, o in enumerate((8192, 1024, 1024))]
+    o_proj = [GpuLayer16(8192, 8192, seed=93)]
+    gate_up = [GpuLayer16(8192, 28672, seed=94 + k) for k in range(2)]
+    down = [GpuLayer16(28672, 8192, seed=96)]
+    qkv2 = [GpuLayer16(8192, o, seed=97 + k) for k, o in enumerate((8192, 1024, 1024))]
+    stages = [qkv, o_proj, gate_up, down, qkv2]
+    assert all(native.lists16_max_tokens([l.desc for l in st]) == 4 for st in stages)
+    for tokens in (1, 3, 4):
+        x0 = torch.randn(tokens, 8192, device="cuda", generator=torch.Generator(device="cuda").manual_seed(tokens))
+        x0 = (0.5 * x0).half()
+        outs = [torch.empty(tokens, sum(l.O for l in st), dtype=torch.float16, device="cuda") for st in stages]
+
+        def views(k):
+            a, v = 0, []
+            for l in stages[k]:
+                v.append(outs[k][:, a:a + l.O])
+                a += l.O
+            return v
+        srcs = [x0, outs[0][:, :8192], outs[1], outs[2][:, :28672], outs[3]]
+        launches = [native.FusedGemvLists16([l.desc for l in st], views(k)) for k, st in enumerate(stages)]
+
+        def chain(flags):
+            for fb, src in zip(launches, srcs):
+                fb(src, flags)
+
+        ref = []
+        for fb, src, out in zip(launches, srcs, outs):          # one at a time, no PDL
+            fb(src, 0)
+            torch.cuda.synchronize()
+            ref.append(out.clone())
+        for o in outs:
+            o.fill_(float("nan"))
+        names = launched_kernels(lambda: chain(native.FLAG_PDL))
+        assert len(names) == 5 and all(ran([n], "gemv_lists16_kernel") for n in names), names
+        assert all(same(o, r) for o, r in zip(outs, ref)), tokens
+        s = torch.cuda.Stream()
+        s.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(s):
+            chain(native.FLAG_PDL)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g, stream=s):
+                chain(native.FLAG_PDL)
+        for o in outs:
+            o.fill_(float("nan"))
+        for _ in range(3):
+            g.replay()
+        torch.cuda.synchronize()
+        for k, (o, r) in enumerate(zip(outs, ref)):
+            assert same(o, r), (tokens, k)
+        for k, st in enumerate(stages):
+            src = x0 if k == 0 else [None, ref[0][:, :8192], ref[1], ref[2][:, :28672], ref[3]][k]
             a = 0
             for l in st:
                 rows = l.sample(16, seed=k)

@@ -14,8 +14,7 @@ import vptq_oracle as vo
 pytestmark = pytest.mark.gpu
 
 from _batch import ZERO_HEAD, assert_close, head_zero, kernel_star, q_of, rand_x
-
-KERNEL = "gemv_lists16_kernel"
+from _lists16 import KERNEL, GpuLayer16, desc_t as _desc_t
 
 CASES = {
     "k65536_r256_fp16": dict(in_features=4096, out_features=1024, num_centroids=65536, num_res_centroids=256),
@@ -52,17 +51,6 @@ def _tensors(L):
                 weight_scale=to_t(L.weight_scale, L) if L.weight_scale is not None else None,
                 weight_bias=to_t(L.weight_bias, L) if L.weight_bias is not None else None,
                 bias=to_t(L.bias, L) if L.bias is not None else None)
-
-
-def _desc_t(t, dtype, I, O, K, Kr, lists16=True):
-    """descriptor of a v = 16 layer (its tensors hang off it as `_tensors`), with or without the v = 16 lists"""
-    from vptq_b200 import native
-    d = native.make_desc(dtype=torch.float16 if dtype == "fp16" else torch.bfloat16, in_features=I, out_features=O,
-                         vector_len=16, num_centroids=K, num_res_centroids=Kr, num_codebooks=1, group_size=I,
-                         outlier_size=0, outlier_vector_len=-1, num_outlier_centroids=-1, outlier_indices=None,
-                         outlier_centroids=None, lists16=lists16, **t)
-    d._tensors = t
-    return d
 
 
 def _desc(L, lists16=True):
@@ -148,53 +136,6 @@ def test_random_x_against_fp64(name):
 
 
 # ---------------------------------------------------------------- full-size layers, checked on sampled rows
-class GpuLayer16:
-    """A seeded v = 16 layer (one group) generated and packed on the GPU, with its v = 16 list descriptor;
-    `check` compares outputs on a sample of index rows with the oracle of those rows."""
-
-    def __init__(self, I, O, *, K=65536, Kr=256, dtype="fp16", seed=0, lists16=True):
-        from vptq_b200.pack import pack_index
-        self.I, self.O, self.K, self.Kr, self.dtype = I, O, K, Kr, dtype
-        self.Ro = (O + 15) // 16
-        dt = torch.float16 if dtype == "fp16" else torch.bfloat16
-        g = torch.Generator(device="cuda").manual_seed(seed)
-        rnd = lambda *s: torch.randn(*s, device="cuda", generator=g)
-        idx = torch.randint(0, K, (1, self.Ro, I), device="cuda", generator=g)
-        ridx = torch.randint(0, Kr, (1, self.Ro, I), device="cuda", generator=g) if Kr > 0 else None
-        t = dict(indices=pack_index(idx, K.bit_length() - 1, ridx, Kr.bit_length() - 1 if Kr > 0 else 0))
-        del idx, ridx
-        t["centroids"] = (0.02 * rnd(1, K * 16)).to(dt)
-        t["res_centroids"] = (0.005 * rnd(1, Kr * 16)).to(dt) if Kr > 0 else None
-        t["perm"] = torch.randperm(I, device="cuda", generator=g).to(torch.int32).to(torch.int16)
-        t["weight_scale"] = (1.0 + 0.1 * rnd(I)).to(dt)
-        t["weight_bias"] = (0.01 * rnd(I)).to(dt)
-        t["bias"] = None
-        self.t = t
-        self.desc = _desc_t(t, dtype, I, O, K, Kr if Kr > 0 else -1, lists16)
-
-    def check(self, x, y, n=48, seed=0):
-        from _batch import _np16
-        import _extreme as ex
-        rows = np.sort(np.append(np.random.default_rng(seed).choice(self.Ro - 1, size=n - 1, replace=False),
-                                 self.Ro - 1))
-        t, dt = self.t, self.dtype
-        cols = (rows[:, None] * 16 + np.arange(16)[None, :]).reshape(-1)
-        keep = cols < self.O
-        L = vo.Layer(dtype=dt, in_features=self.I, out_features=len(rows) * 16, vector_len=16, num_centroids=self.K,
-                     num_res_centroids=self.Kr, num_codebooks=1, group_size=self.I)
-        L.indices = t["indices"][:, torch.from_numpy(rows).cuda()].cpu().numpy()
-        L.centroids = _np16(t["centroids"], dt)
-        L.res_centroids = _np16(t["res_centroids"], dt)
-        L.perm = t["perm"].cpu().numpy().view(np.uint16)
-        L.weight_scale, L.weight_bias = _np16(t["weight_scale"], dt), _np16(t["weight_bias"], dt)
-        k = torch.from_numpy(np.nonzero(keep)[0]).cuda()
-        ys = y[:, torch.from_numpy(cols[keep]).cuda()]
-        q = q_of(self.I, self.K)
-        assert torch.isfinite(ys).all()
-        assert_close(ys, kernel_star(L, x)[:, k], dt, q)
-        assert_close(ys, ex.y_star(L, x)[:, k], dt, q, factor=2.0)
-
-
 FULL = {   # (in_features, [out_features of the fused members]): Llama-3-70B / Nemotron-70B and Llama-3.1-405B
     "70b_qkv": (8192, [8192, 1024, 1024]), "70b_o": (8192, [8192]), "70b_gate_up": (8192, [28672, 28672]),
     "70b_down": (28672, [8192]), "405b_q": (16384, [16384]), "405b_o": (16384, [16384]),

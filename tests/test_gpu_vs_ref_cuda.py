@@ -134,3 +134,75 @@ def test_dequant_matches_reference_cuda(ref, name):
     bound = 2 * ulp * (np.abs(W_ref) + wb) + 1e-7
     bad = np.abs(W - W_ref) > bound
     assert not bad.any(), f"{int(bad.sum())} of {bad.size} sampled elements beyond the double-rounding bound"
+
+
+# ------------------------------------------------------------------------------------------------ vector length 16
+# The reference's quant_gemv dispatches group size 16 with 16 index bits and 8 (or no) residual bits.  Its outputs on
+# these cases are in tests/golden/ref_cuda/v16.npz (oracle/make_ref_cuda_golden.py --v16); outputs.npz is unchanged.
+REF16_GOLDEN = os.path.join(GOLDEN_DIR, "ref_cuda", "v16.npz")
+V16_CASES = {
+    "v16_k65536_r256": dict(in_features=4096, out_features=1024, vector_len=16, num_centroids=65536,
+                            num_res_centroids=256),
+    "v16_k65536_r256_bf16": dict(in_features=4096, out_features=1024, vector_len=16, num_centroids=65536,
+                                 num_res_centroids=256, dtype="bf16"),
+    "v16_k65536_r0": dict(in_features=2048, out_features=1024, vector_len=16, num_centroids=65536),
+}
+V16_DEQUANT_CASES = ["v16_k65536_r256", "v16_k65536_r256_bf16"]
+
+
+@pytest.fixture(scope="module")
+def ref16():
+    return np.load(REF16_GOLDEN, allow_pickle=False)
+
+
+@pytest.mark.parametrize("route", ["default", "lists16"])
+@pytest.mark.parametrize("name", sorted(V16_CASES))
+def test_v16_gemv_matches_reference_cuda(ref16, name, route):
+    """the default v = 16 route (the generic GEMV) and the v = 16 list kernel (set_list_decode) at 1 and 2 tokens
+    against the record, with the bars of test_gemv_matches_reference_cuda"""
+    import torch
+    from _gpu import from_t, make_module, x_to_t
+    from _probe import launched_kernels, ran
+    L = vo.make_layer(seed=GEMV_SEED, **V16_CASES[name])
+    m = make_module(L)
+    if route == "lists16":
+        m.set_list_decode(True)
+    tol = 1e-3 if L.dtype == "fp16" else 8e-3
+    for tokens in (1, 2):
+        x_np = vo.make_x(tokens, L.in_features, L.dtype, seed=tokens)
+        x = x_to_t(x_np, L)
+        with torch.no_grad():
+            m(x)
+            names = launched_kernels(lambda: m(x))
+            assert ran(names, "gemv_lists16_kernel") == (route == "lists16"), names
+            y_ours = from_t(m(x))
+        y_ref = from_bits(ref16[f"gemv__{name}__t{tokens}"], L.dtype)
+        torch.cuda.synchronize()
+        y_star = vo.quant_gemm(x_np, L)
+        e_ours = parity_error(y_ours, y_star)
+        assert e_ours <= tol
+        if not np.isfinite(y_ref).all():
+            print(f"{name} {route} tokens={tokens}: ours-vs-exact {e_ours:.2e}  reference kernel output is not finite, "
+                  "skipped")
+            continue
+        assert y_ours.shape == y_ref.shape
+        e_ref, e_mut = parity_error(y_ref, y_star), parity_error(y_ours, y_ref)
+        print(f"{name} {route} tokens={tokens}: ours-vs-exact {e_ours:.2e}  ref-vs-exact {e_ref:.2e}  "
+              f"ours-vs-ref {e_mut:.2e}")
+        assert e_mut <= max(tol, 2 * e_ref), (e_mut, e_ref)
+
+
+@pytest.mark.parametrize("name", V16_DEQUANT_CASES)
+def test_v16_dequant_matches_reference_cuda(ref16, name):
+    from _gpu import from_t, make_module
+    L = vo.make_layer(seed=DEQUANT_SEED, **V16_CASES[name])
+    m = make_module(L)
+    W = from_t(m.dequant())
+    assert W.shape == tuple(ref16[f"dequant__{name}__shape"])
+    W = W.reshape(-1)[sample_positions(W.size)]
+    W_ref = from_bits(ref16[f"dequant__{name}__values"], L.dtype)
+    ulp = 2.0 ** -10 if L.dtype == "fp16" else 2.0 ** -7
+    wb = np.abs(vo.to_f32(L.weight_bias, L.dtype)).max()
+    bound = 2 * ulp * (np.abs(W_ref) + wb) + 1e-7
+    bad = np.abs(W - W_ref) > bound
+    assert not bad.any(), f"{int(bad.sum())} of {bad.size} sampled elements beyond the double-rounding bound"

@@ -308,6 +308,60 @@ def test_limits_and_the_max_tokens_rule():
     assert not lists.launchable(53248, 65536, SM_COUNT) and lists.launchable(28672, 65536, SM_COUNT)
 
 
+def _plan(I, outs, Kr=256):
+    """(carve of each instance 1, 2, 4, max_tokens) of the fused layers `outs` at in_features I"""
+    ns, nt, tcw = lists.geometry(I, 65536)
+    Ro = [(o + 15) // 16 for o in outs]
+    k = partition(Ro, ns * nt)
+    mn = max((r + kl - 1) // kl for r, kl in zip(Ro, k))
+    return {n: carve(tcw, mn, Kr, n) for n in (1, 2, 4)}, max_tokens(I, outs, Kr=Kr)
+
+
+def test_cut_off_shapes_of_the_gpu_envelope():
+    """every shape tests/test_gpu_lists16_envelope.py runs at a cut-off (tests/_lists16.py), on its side of it"""
+    import _lists16 as l16
+    assert (SM_COUNT, SMEM_OPTIN) == (l16.SM_COUNT, l16.SMEM_OPTIN)
+    # one shape per (replication, stages) the carve chooses, at the instance of its token count
+    for (rep, stages), (I, O, Kr, tokens) in l16.CARVE.items():
+        c, mt = _plan(I, [O], Kr)
+        assert c[4 if tokens > 2 else tokens][1:] == (rep, stages) and mt == 4, (rep, stages)
+    assert _plan(4096, [1024], 0)[0] == {1: (191616, 8, 3), 2: (201856, 8, 3), 4: (222336, 8, 3)}
+    assert _plan(4096, [1024], 64)[0][4] == (222208, 8, 2)
+    assert _plan(4096, [1024])[0] == {1: (224384, 4, 3), 2: (218112, 4, 2), 4: (222208, 2, 2)}
+    # the carve never chooses 3 stages below replication 4 for Kr <= 256 (dropping a stage frees at least as much)
+    for Kr in (0, 2, 64, 128, 256):
+        for tcw in (1024, 2056, 3008, 4096):
+            for mn in (1, 8, 257, 1024, 3328, 4511, 4512, 8192):
+                for ntok in (1, 2, 4):
+                    assert carve(tcw, mn, Kr, ntok)[1:] not in ((2, 3), (1, 3))
+    # the exact fit: I = 32768 (Q = 128, B = 1), out = 72176 fills the opt-in at NTOK = 4 with replication 1;
+    # one index row more (72192) does not fit at 4 tokens and takes 2 (replication 2 there)
+    assert partition([l16.EXACT_FIT[1] // 16], 128) == [1] and lists.geometry(32768, 65536)[:2] == (16, 8)
+    c, mt = _plan(*l16.EXACT_FIT[:1], [l16.EXACT_FIT[1]])
+    assert c[4] == (232448, 1, 2) and mt == 4
+    assert carve(4096, 4511, 256, 4, limit=SMEM_OPTIN - 1) == (0, 0, 0)
+    c, mt = _plan(*l16.PAST_FIT[:1], [l16.PAST_FIT[1]])
+    assert c[4] == (0, 0, 0) and c[2] == (220288, 2, 2) and mt == 2
+    assert carve(4096, 4512, 256, 4, limit=SMEM_OPTIN + 128) == (SMEM_OPTIN + 128, 1, 2)
+    # the row-token limit at I = 4096 (Q = 16, B = 8): 32768 [row][token] accumulators of 16 outputs
+    for O, want in l16.ROW_TOKENS.items():
+        assert max_tokens(4096, [O]) == want, O
+        rows = (O + 15) // 16
+        assert rows * want <= MAX_ROW_TOKENS and (want == 4 or rows * max(2 * want, 1) > MAX_ROW_TOKENS), O
+    assert (524288 // 16) * 1 == MAX_ROW_TOKENS                     # 1 token: the head exactly full
+    assert _plan(4096, [524288])[0][1][0] > 0                        # (the 1-token layout fits)
+    # the fused 405B q/k/v: three layers, B = 2; each member alone takes 4 tokens
+    I, outs = l16.QKV_405B
+    assert lists.geometry(I, 65536)[:2] == (16, 4) and partition([o // 16 for o in outs], 64) is None
+    assert max_tokens(I, outs) == 0 and all(max_tokens(I, [o]) == 4 for o in outs)
+    # partition extremes: B = 1 at I = 32768; one row per CTA at I = 4096, out = 128; Ro = 1
+    assert partition([256], 128) == [1] and partition([8], 16) == [8] and partition([1], 16) == [1]
+    runs = kernel_split([8], 16, [[s for s in range(0, 16 * 8 + 1)]])         # (1-step units: 15 warps idle)
+    assert all(sum(b > a for a, b in w) == 1 for *_, w in runs)
+    runs = kernel_split([8], 16, [[0] + [128 * (i + 1) for i in range(16 * 8)]])   # 128-step units: all 16 busy
+    assert all(all(b - a == 8 for a, b in w) for *_, w in runs)
+
+
 def test_partition_does_not_depend_on_the_token_count():
     """the kernel's split takes no token argument at all: the mirror above has none, and neither has
     lists16_partition (only the shared-memory carve and the accumulator offsets see the instance)"""
