@@ -14,6 +14,13 @@
  * aligned with a row pitch that is a multiple of 8, VPTQ_B200_GEMM_PREP unset) and for every input gradient, results
  * are bit-identical to it.  Elsewhere they agree to within the prefill route's rounding (x is not pre-scaled here).
  *
+ * Both list geometries are taken: vector_len 8 (the lists of vptq_b200_quant_gemv) and vector_len 16 (the lists of
+ * vptq_b200_quant_gemv_lists16, include/vptq_b200_lists16.h: an index row covers 16 outputs, lists_tile_cols of
+ * that header's geometry).  Either way one codebook group, no outliers, K = 4096 * (2..16) and Kr <= 256.  The
+ * workspace layout is the same for both: W [out_features][in_features rounded up to 64] (Wt: [in_features][pitch of
+ * the input-gradient GEMM]) after the zero-at-rest head, then the staged activation.  At vector_len 16 the last index
+ * row's outputs past out_features are never part of W, and are zeros in Wt.
+ *
  * Every call accepts a descriptor that carries index lists, decode-only or full (the packed words are then
  * ignored), and refuses one without them (VPTQ_ERR_UNSUPPORTED).  Conventions are those of include/vptq_b200.h: the
  * caller allocates outputs and workspace (zero-initialised once; kernels leave its head zeroed), no call allocates

@@ -157,7 +157,8 @@ int need_packed(const vptq_linear_desc* d, const char* what) {
   return VPTQ_ERR_UNSUPPORTED;
 }
 
-// calls of include/vptq_b200_lists_dense.h: a descriptor whose index lists the list kernels take, full or decode-only
+// calls of include/vptq_b200_lists_dense.h: a descriptor whose index lists the list kernels take (vector length 8 or
+// 16), full or decode-only
 int validate_lists(const vptq_linear_desc* d, uint32_t flags, uint32_t allowed_flags, const char* what) {
   if (int rc = validate(d, false)) return rc;
   if (flags & ~allowed_flags) {
@@ -168,10 +169,10 @@ int validate_lists(const vptq_linear_desc* d, uint32_t flags, uint32_t allowed_f
     set_error("%s: this descriptor carries no index lists (lists_stream / lists_tab are NULL)", what);
     return VPTQ_ERR_UNSUPPORTED;
   }
-  if (!gemv_lists_eligible(*d)) {
-    set_error("%s: index lists of a layer the list kernels do not take (vector_len 8, one codebook group, no outliers, "
-              "K = 4096 * (2..16), Kr <= 256, lists_tile_cols of the lists geometry, 16-byte aligned lists_stream, "
-              "weight_scale and weight_bias)", what);
+  if (!gemv_lists_eligible(*d) && !gemv_lists16_eligible(*d)) {
+    set_error("%s: index lists of a layer the list kernels do not take (vector_len 8 or 16, one codebook group, no "
+              "outliers, K = 4096 * (2..16), Kr <= 256, lists_tile_cols of the lists geometry of that vector length, "
+              "16-byte aligned lists_stream, weight_scale and weight_bias)", what);
     return VPTQ_ERR_UNSUPPORTED;
   }
   return 0;

@@ -136,7 +136,8 @@ bool dequant_orig_fast_ok(const vptq_linear_desc& d, const void* w_out, int64_t 
 int dequant_transposed_launch(const vptq_linear_desc& d, void* wt_out, int64_t ld, cudaStream_t stream);
 
 // the same W (transposed: Wt) from the index lists (lists_dense.cu, C interface include/vptq_b200_lists_dense.h):
-// layers with gemv_lists_eligible(d), out 16-byte aligned, ld % 8 == 0, ld >= in_features (Wt: >= out_features)
+// layers with gemv_lists_eligible(d) or gemv_lists16_eligible(d), out 16-byte aligned, ld % 8 == 0, ld >= in_features
+// (Wt: >= out_features)
 int lists_dense_launch(const vptq_linear_desc& d, void* out, int64_t ld, bool transposed, cudaStream_t stream);
 
 // -------------------------------------------------------------------------------------------

@@ -12,15 +12,20 @@
 // float(wbias[f])) rounded once to the layer type, scale 1 and bias 0 without a norm, so W and Wt are bit-identical
 // to vptq_b200_dequant and to the transposed dequant of the input-gradient GEMM.
 //
+// Vector length V = 8 (gemv_lists_eligible) or 16 (gemv_lists16_eligible): an index row covers V outputs, an entry
+// is V elements -- H = V / 8 halves of 8, each one 16-byte codebook gather, residual read and store.
+//
 // Work split: one CTA per (index row r, tile t), 256 threads.  The steps of the NS units are laid end to end and
 // dealt to the 8 warps step by step (LD_UNROLL steps in flight per warp: 8 independent 16-byte codebook gathers
 // per lane), so skewed slices do not leave warps idle.  Residual entries come from a bank-replicated shared-memory
-// table (copy k of entry i at slot 8 i + k, lane L reads copy L & 7), as in dequant.cu's fast paths.
-//   * original order W[o][f]: each entry's 8 results (outputs 8r..8r+7 of feature f) go to a [TCW][8] shared tile
-//     (feature slots XOR-swizzled by (f >> 3) & 7); after a barrier a thread owns 8 consecutive features, transposes
-//     the 8x8 block in registers and writes one 16-byte vector per output row.
-//   * transposed Wt[f][o]: an entry is 8 consecutive elements of Wt row f, written as one 16-byte store; CTAs of
-//     index rows past Ro write the zero columns [8 Ro, ld).
+// table (copy k of half h of entry i at slot 8 (H i + h) + k, lane L reads copy L & 7), as in dequant.cu's fast
+// paths.
+//   * original order W[o][f]: half h of each entry's results (outputs V r + 8 h .. + 7 of feature f) goes to plane h
+//     of H [TCW][8] shared tiles (feature slots XOR-swizzled by (f >> 3) & 7); after a barrier a thread owns 8
+//     consecutive features, transposes each plane's 8x8 block in registers and writes one 16-byte vector per output
+//     row.  At V = 16, TCW <= 4096: 128 KiB of planes + 64 KiB of residual table at Kr = 256.
+//   * transposed Wt[f][o]: an entry is V consecutive elements of Wt row f, written as H 16-byte stores (outputs past
+//     O as zeros, halves at or past ld skipped); CTAs of index rows past Ro write the zero columns [V Ro, ld).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -43,8 +48,9 @@ struct ListsDenseParams {
   int I, O, Ro, NS, TCW, Kr;
 };
 
-template <typename T, bool TR>
+template <typename T, bool TR, int V>
 __global__ void __launch_bounds__(LD_THREADS) lists_dense_kernel(const __grid_constant__ ListsDenseParams p) {
+  constexpr int H = V / 8;
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ uint32_t s_first[LD_MAX_SLICES + 1], s_step0[LD_MAX_SLICES], s_nsteps[LD_MAX_SLICES],
       s_valid[LD_MAX_SLICES];
@@ -53,9 +59,12 @@ __global__ void __launch_bounds__(LD_THREADS) lists_dense_kernel(const __grid_co
   const int f0 = t * p.TCW, ncols = min(p.TCW, p.I - f0);
   T* out = reinterpret_cast<T*>(p.out);
 
-  if (TR && r >= p.Ro) {  // the zero K tail of Wt: columns [8 Ro, ld) of the tile's rows
-    for (int f = tid; f < ncols; f += LD_THREADS)
-      *reinterpret_cast<uint4*>(out + int64_t(f0 + f) * p.ld + int64_t(r) * 8) = make_uint4(0u, 0u, 0u, 0u);
+  if (TR && r >= p.Ro) {  // the zero K tail of Wt: columns [V Ro, ld) of the tile's rows
+    for (int h = 0; h < H; ++h) {
+      if (V > 8 && int64_t(r) * V + 8 * h >= p.ld) break;
+      for (int f = tid; f < ncols; f += LD_THREADS)
+        *reinterpret_cast<uint4*>(out + int64_t(f0 + f) * p.ld + int64_t(r) * V + 8 * h) = make_uint4(0u, 0u, 0u, 0u);
+    }
     return;
   }
 
@@ -66,9 +75,9 @@ __global__ void __launch_bounds__(LD_THREADS) lists_dense_kernel(const __grid_co
     s_nsteps[tid] = (b & LD_STEP_MASK) - (a & LD_STEP_MASK);
     s_valid[tid] = a >> 26;
   }
-  uint8_t* s_res = smem;                                   // [Kr][8] replicated 16-byte entries
-  uint8_t* s_tile = smem + size_t(p.Kr) * 128;             // [TCW][8] results (original order only)
-  for (int slot = tid; slot < p.Kr * 8; slot += LD_THREADS)
+  uint8_t* s_res = smem;                                   // [Kr][H][8] replicated 16-byte halves
+  uint8_t* s_tile = smem + size_t(p.Kr) * 128 * H;         // H x [TCW][8] results (original order only)
+  for (int slot = tid; slot < p.Kr * 8 * H; slot += LD_THREADS)
     sts_v4(smem_u32(s_res) + uint32_t(slot) * 16u,
            ldg_nc_v4(reinterpret_cast<const uint8_t*>(p.res_centroids) + size_t(slot >> 3) * 16, policy_evict_last()));
   __syncthreads();
@@ -85,7 +94,7 @@ __global__ void __launch_bounds__(LD_THREADS) lists_dense_kernel(const __grid_co
   const T* wbias = reinterpret_cast<const T*>(p.wbias);
   const uint32_t res_lane = smem_u32(s_res) + (lane & 7) * 16;
   const uint64_t keep = policy_evict_last();
-  const int o0 = r * 8;
+  const int o0 = r * V;
 
   for (uint32_t base = warp; base < total; base += LD_WARPS * LD_UNROLL) {
     uint32_t ent[LD_UNROLL], sl[LD_UNROLL];
@@ -103,74 +112,87 @@ __global__ void __launch_bounds__(LD_THREADS) lists_dense_kernel(const __grid_co
         if (ok[i]) ent[i] = ldg_nc_u32(p.stream + (size_t(s_step0[s]) + k) * 32 + lane);
       }
     }
-    uint4 cw[LD_UNROLL];
+    uint4 cw[LD_UNROLL][H];
 #pragma unroll
     for (int i = 0; i < LD_UNROLL; ++i)
-      cw[i] = ok[i] ? ldg_nc_v4(cb + (size_t(sl[i] << 12) | (ent[i] & 4095u)) * 16, keep) : make_uint4(0u, 0u, 0u, 0u);
+#pragma unroll
+      for (int h = 0; h < H; ++h)
+        cw[i][h] = ok[i] ? ldg_nc_v4(cb + (size_t(sl[i] << 12) | (ent[i] & 4095u)) * (16 * H) + 16 * h, keep)
+                         : make_uint4(0u, 0u, 0u, 0u);
 #pragma unroll
     for (int i = 0; i < LD_UNROLL; ++i) {
       if (!ok[i]) continue;
       const int col = int((ent[i] >> 12) & 4095u), f = f0 + col;
       const float sc = scale ? DT<T>::to_float(scale[f]) : 1.f, wb = scale ? DT<T>::to_float(wbias[f]) : 0.f;
-      uint4 rw = make_uint4(0u, 0u, 0u, 0u);
-      if (p.Kr) rw = lds_v4(res_lane + (ent[i] >> 24) * 128);
-      const uint32_t cwk[4] = {cw[i].x, cw[i].y, cw[i].z, cw[i].w}, rwk[4] = {rw.x, rw.y, rw.z, rw.w};
-      uint32_t hv[4];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float2 c2 = DT<T>::unpack2(cwk[j]);
-        if (p.Kr) {
-          const float2 r2 = DT<T>::unpack2(rwk[j]);
-          c2.x += r2.x, c2.y += r2.y;
+      for (int h = 0; h < H; ++h) {
+        uint4 rw = make_uint4(0u, 0u, 0u, 0u);
+        if (p.Kr) rw = lds_v4(res_lane + (ent[i] >> 24) * (128 * H) + 128 * h);
+        const uint32_t cwk[4] = {cw[i][h].x, cw[i][h].y, cw[i][h].z, cw[i][h].w}, rwk[4] = {rw.x, rw.y, rw.z, rw.w};
+        uint32_t hv[4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          float2 c2 = DT<T>::unpack2(cwk[j]);
+          if (p.Kr) {
+            const float2 r2 = DT<T>::unpack2(rwk[j]);
+            c2.x += r2.x, c2.y += r2.y;
+          }
+          hv[j] = DT<T>::pack2(fmaf(c2.x, sc, wb), fmaf(c2.y, sc, wb));
+          if (TR) {  // outputs past O (padding rows of the last index row): zeros
+            const int o = o0 + 8 * h + 2 * j;
+            if (o >= p.O) hv[j] = 0u;
+            else if (o + 1 >= p.O) hv[j] &= 0xffffu;
+          }
         }
-        hv[j] = DT<T>::pack2(fmaf(c2.x, sc, wb), fmaf(c2.y, sc, wb));
-        if (TR) {  // outputs past O (padding rows of the last index row): zeros
-          const int o = o0 + 2 * j;
-          if (o >= p.O) hv[j] = 0u;
-          else if (o + 1 >= p.O) hv[j] &= 0xffffu;
+        if (TR) {
+          if (V > 8 && o0 + 8 * h >= p.ld) break;  // a last half wholly past ld (ld % 16 == 8): all padding
+          *reinterpret_cast<uint4*>(out + int64_t(f) * p.ld + o0 + 8 * h) = make_uint4(hv[0], hv[1], hv[2], hv[3]);
+        } else {
+          const uint32_t slot = uint32_t(col) ^ ((uint32_t(col) >> 3) & 7u);
+          sts_v4(smem_u32(s_tile) + uint32_t(h * p.TCW) * 16u + slot * 16u, make_uint4(hv[0], hv[1], hv[2], hv[3]));
         }
-      }
-      if (TR) {
-        *reinterpret_cast<uint4*>(out + int64_t(f) * p.ld + o0) = make_uint4(hv[0], hv[1], hv[2], hv[3]);
-      } else {
-        const uint32_t slot = uint32_t(col) ^ ((uint32_t(col) >> 3) & 7u);
-        sts_v4(smem_u32(s_tile) + slot * 16u, make_uint4(hv[0], hv[1], hv[2], hv[3]));
       }
     }
   }
   if (TR) return;
   __syncthreads();
 
-  // 8 consecutive features per thread: 8x8 register transpose, one 16-byte store per output row
-  const int rows = min(8, p.O - o0);  // padding rows are never written
-  for (int j = tid; j * 8 < ncols; j += LD_THREADS) {
-    uint32_t hv[8][4];
+  // 8 consecutive features per thread: per plane an 8x8 register transpose, one 16-byte store per output row
+  const int rows = min(V, p.O - o0);  // padding rows are never written
+  for (int h = 0; h < H; ++h) {
+    const int rh = H == 1 ? rows : min(8, rows - 8 * h);  // rows of plane h
+    if (V > 8 && rh <= 0) break;
+    const uint32_t plane = smem_u32(s_tile) + uint32_t(h * p.TCW) * 16u;
+    const int oh = o0 + 8 * h;
+    for (int j = tid; j * 8 < ncols; j += LD_THREADS) {
+      uint32_t hv[8][4];
 #pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const uint4 v = lds_v4(smem_u32(s_tile) + uint32_t(j * 8 + (k ^ (j & 7))) * 16u);
-      hv[k][0] = v.x, hv[k][1] = v.y, hv[k][2] = v.z, hv[k][3] = v.w;
-    }
-    const int fb = f0 + j * 8;
-    if (j * 8 + 8 <= ncols) {
-#pragma unroll
-      for (int e = 0; e < 8; ++e) {
-        if (e >= rows) break;
-        const uint32_t sel = (e & 1) ? 0x7632u : 0x5410u;
-        uint4 v;
-        v.x = __byte_perm(hv[0][e >> 1], hv[1][e >> 1], sel);
-        v.y = __byte_perm(hv[2][e >> 1], hv[3][e >> 1], sel);
-        v.z = __byte_perm(hv[4][e >> 1], hv[5][e >> 1], sel);
-        v.w = __byte_perm(hv[6][e >> 1], hv[7][e >> 1], sel);
-        *reinterpret_cast<uint4*>(out + int64_t(o0 + e) * p.ld + fb) = v;
+      for (int k = 0; k < 8; ++k) {
+        const uint4 v = lds_v4(plane + uint32_t(j * 8 + (k ^ (j & 7))) * 16u);
+        hv[k][0] = v.x, hv[k][1] = v.y, hv[k][2] = v.z, hv[k][3] = v.w;
       }
-    } else {  // the last tile's ragged end (in_features % 8 != 0)
-      uint16_t* o16 = reinterpret_cast<uint16_t*>(p.out);
+      const int fb = f0 + j * 8;
+      if (j * 8 + 8 <= ncols) {
 #pragma unroll
-      for (int k = 0; k < 8; ++k)
+        for (int e = 0; e < 8; ++e) {
+          if (e >= rh) break;
+          const uint32_t sel = (e & 1) ? 0x7632u : 0x5410u;
+          uint4 v;
+          v.x = __byte_perm(hv[0][e >> 1], hv[1][e >> 1], sel);
+          v.y = __byte_perm(hv[2][e >> 1], hv[3][e >> 1], sel);
+          v.z = __byte_perm(hv[4][e >> 1], hv[5][e >> 1], sel);
+          v.w = __byte_perm(hv[6][e >> 1], hv[7][e >> 1], sel);
+          *reinterpret_cast<uint4*>(out + int64_t(oh + e) * p.ld + fb) = v;
+        }
+      } else {  // the last tile's ragged end (in_features % 8 != 0)
+        uint16_t* o16 = reinterpret_cast<uint16_t*>(p.out);
 #pragma unroll
-        for (int e = 0; e < 8; ++e)
-          if (k < ncols - j * 8 && e < rows)
-            o16[int64_t(o0 + e) * p.ld + fb + k] = uint16_t(hv[k][e >> 1] >> ((e & 1) * 16));
+        for (int k = 0; k < 8; ++k)
+#pragma unroll
+          for (int e = 0; e < 8; ++e)
+            if (k < ncols - j * 8 && e < rh)
+              o16[int64_t(oh + e) * p.ld + fb + k] = uint16_t(hv[k][e >> 1] >> ((e & 1) * 16));
+      }
     }
   }
   if (f0 + ncols == p.I) {  // the last tile's CTAs write the zero columns [I, ld) of their rows
@@ -183,8 +205,30 @@ __global__ void __launch_bounds__(LD_THREADS) lists_dense_kernel(const __grid_co
 }  // namespace
 
 size_t lists_dense_smem_bytes(const vptq_linear_desc& d, bool transposed) {
-  const size_t res = d.num_res_centroids > 0 ? size_t(d.num_res_centroids) * 128 : 0;
-  return res + (transposed ? 0 : size_t(d.lists_tile_cols) * 16);
+  const size_t H = d.vector_len / 8;
+  const size_t res = d.num_res_centroids > 0 ? size_t(d.num_res_centroids) * 128 * H : 0;
+  return res + (transposed ? 0 : size_t(d.lists_tile_cols) * 16 * H);
+}
+
+template <int V>
+int lists_dense_launch_v(const ListsDenseParams& p, int dtype, bool transposed, dim3 grid, size_t smem,
+                         cudaStream_t stream) {
+  const void* fn;
+  if (dtype == VPTQ_FP16)
+    fn = transposed ? reinterpret_cast<const void*>(lists_dense_kernel<__half, true, V>)
+                    : reinterpret_cast<const void*>(lists_dense_kernel<__half, false, V>);
+  else
+    fn = transposed ? reinterpret_cast<const void*>(lists_dense_kernel<__nv_bfloat16, true, V>)
+                    : reinterpret_cast<const void*>(lists_dense_kernel<__nv_bfloat16, false, V>);
+  if (int rc = ensure_smem_attr(fn, (V == 8 ? 100 : 200) * 1024)) return rc;
+  if (dtype == VPTQ_FP16) {
+    if (transposed) lists_dense_kernel<__half, true, V><<<grid, LD_THREADS, smem, stream>>>(p);
+    else lists_dense_kernel<__half, false, V><<<grid, LD_THREADS, smem, stream>>>(p);
+  } else {
+    if (transposed) lists_dense_kernel<__nv_bfloat16, true, V><<<grid, LD_THREADS, smem, stream>>>(p);
+    else lists_dense_kernel<__nv_bfloat16, false, V><<<grid, LD_THREADS, smem, stream>>>(p);
+  }
+  return 0;
 }
 
 int lists_dense_launch(const vptq_linear_desc& d, void* out, int64_t ld, bool transposed, cudaStream_t stream) {
@@ -193,27 +237,16 @@ int lists_dense_launch(const vptq_linear_desc& d, void* out, int64_t ld, bool tr
   p.centroids = d.centroids, p.res_centroids = d.res_centroids;
   p.scale = d.weight_scale, p.wbias = d.weight_scale ? d.weight_bias : nullptr;
   p.out = out, p.ld = ld;
-  p.I = d.in_features, p.O = d.out_features, p.Ro = (d.out_features + 7) / 8;
+  const int V = d.vector_len;  // 8 or 16: the caller checked gemv_lists_eligible or gemv_lists16_eligible
+  p.I = d.in_features, p.O = d.out_features, p.Ro = (d.out_features + V - 1) / V;
   p.NS = d.num_centroids / 4096, p.TCW = d.lists_tile_cols;
   p.Kr = d.num_res_centroids > 0 ? d.num_res_centroids : 0;
   const int nt = (d.in_features + p.TCW - 1) / p.TCW;
   const size_t smem = lists_dense_smem_bytes(d, transposed);
-  dim3 grid(unsigned(transposed ? ld / 8 : p.Ro), unsigned(nt));
-  const void* fn;
-  if (d.dtype == VPTQ_FP16)
-    fn = transposed ? reinterpret_cast<const void*>(lists_dense_kernel<__half, true>)
-                    : reinterpret_cast<const void*>(lists_dense_kernel<__half, false>);
-  else
-    fn = transposed ? reinterpret_cast<const void*>(lists_dense_kernel<__nv_bfloat16, true>)
-                    : reinterpret_cast<const void*>(lists_dense_kernel<__nv_bfloat16, false>);
-  if (int rc = ensure_smem_attr(fn, 100 * 1024)) return rc;
-  if (d.dtype == VPTQ_FP16) {
-    if (transposed) lists_dense_kernel<__half, true><<<grid, LD_THREADS, smem, stream>>>(p);
-    else lists_dense_kernel<__half, false><<<grid, LD_THREADS, smem, stream>>>(p);
-  } else {
-    if (transposed) lists_dense_kernel<__nv_bfloat16, true><<<grid, LD_THREADS, smem, stream>>>(p);
-    else lists_dense_kernel<__nv_bfloat16, false><<<grid, LD_THREADS, smem, stream>>>(p);
-  }
+  dim3 grid(unsigned(transposed ? (ld + V - 1) / V : p.Ro), unsigned(nt));
+  if (int rc = V == 16 ? lists_dense_launch_v<16>(p, d.dtype, transposed, grid, smem, stream)
+                       : lists_dense_launch_v<8>(p, d.dtype, transposed, grid, smem, stream))
+    return rc;
   const cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) {
     set_error("lists dense weight launch: %s", cudaGetErrorString(e));

@@ -26,7 +26,8 @@ member takes its own forward.
 
 `set_lists_prefill(model)` lets decode-only layers (`prepare(drop_packed=True)`) serve prompts from their index lists
 (include/vptq_b200_lists_dense.h).  The generic fused launch cannot take 2-token calls of such a group, so those go to
-each member's own forward.
+each member's own forward.  A decode-only vector-length-16 group (set_list_decode too) only ever launches the v = 16
+list kernel; every call it declines goes to each member's own forward, which never needs the packed words either.
 """
 from __future__ import annotations
 
@@ -67,7 +68,13 @@ class FusedGroup:
     def _descs(self, x: torch.Tensor):
         for l in self.layers:     # (re)build stale descriptors through the layer's own cache logic
             t = l._tensors()
-            if l._cache_key(t, x.dtype, x.device) != l._desc_key or not l._desc_cache:
+            key = l._cache_key(t, x.dtype, x.device)
+            stale = key != l._desc_key
+            if stale and l._decode_only() and l._desc_key is not None:
+                # a decode-only layer's descriptor no longer follows `indices` (its forward keeps it the same way):
+                # only another dtype or device makes it stale, and its forward then refuses the call
+                stale = key[-2:] != l._desc_key[-2:]
+            if stale or not l._desc_cache:
                 l.prepare(x.dtype)
         return [l._desc_cache[0] for l in self.layers]
 

@@ -244,7 +244,14 @@ class VQuantLinear(nn.Module):
         call; every other call -> the GEMM from the lists.  The weight is bit-identical to the packed dequant's, so
         `dequant()`, the input gradient and prefill calls that a full module serves by its prep-free GEMM give the
         full module's results bit for bit.  On a module that still has its packed words nothing changes.  Weight
-        gradients (`set_quant_grad`) and saving the state_dict stay refused on a decode-only module."""
+        gradients (`set_quant_grad`) and saving the state_dict stay refused on a decode-only module.
+
+        Together with `set_list_decode()` it also lets a vector-length-16 layer become decode-only (both before
+        `prepare(drop_packed=True)`): 1..max tokens then run the v = 16 list kernel and every other call, `dequant()`
+        and the input gradient the GEMM from its lists.  Such a module refuses to turn either opt-in off and to save its
+        state_dict (the checkpoint would lack the packed words)."""
+        if not enabled:
+            self._check_v16_opt_ins_kept("set_lists_prefill(False)")
         self._lists_prefill = bool(enabled)
         return self
 
@@ -255,13 +262,16 @@ class VQuantLinear(nn.Module):
         (include/vptq_b200_lists16.h), which stages each 4096-entry codebook slice in shared memory instead of
         gathering the codebook through L1/L2.  Larger calls are routed as without the opt-in.  Its results may differ
         from the default routes in the low-order bits; each token's outputs do not depend on the other tokens of the
-        call.  Backward is unchanged (the packed words are kept; `prepare(drop_packed=True)` stays refused).
+        call.  Backward is unchanged.  With `set_lists_prefill()` as well, `prepare(drop_packed=True)` frees the packed
+        words (decode-only: 4.25 instead of 7.25 bytes per index resident); without it that stays refused.
 
         Only eligible layers change: vector_len 16, one codebook group, no outlier columns, K = 4096 * (2..16),
         Kr <= 256 and slices x column tiles <= the SM count.  On every other layer (v = 8 included) this does
         nothing.  Turning it on drops a descriptor built without the lists (the next call or `prepare()` builds them):
         call it before capturing CUDA graphs."""
         enabled = bool(enabled)
+        if not enabled:
+            self._check_v16_opt_ins_kept("set_list_decode(False)")
         if enabled and not self._list_decode and self.vector_len == 16 and self._desc_cache and \
                 not self._desc_cache[0].lists_stream:
             self._desc_cache, self._desc_key = [], None
@@ -270,6 +280,12 @@ class VQuantLinear(nn.Module):
 
     def _decode_only(self) -> bool:
         return getattr(self, "_drop_packed", False) and self.indices.numel() == 0
+
+    def _check_v16_opt_ins_kept(self, what: str) -> None:
+        # a decode-only v = 16 module has no route for its calls without both list opt-ins
+        if self.vector_len == 16 and self._decode_only():
+            raise RuntimeError(f"{what}: this vector-length-16 VQuantLinear is decode-only (prepare(drop_packed=True)) "
+                               "and serves its calls from its index lists only; reload the checkpoint first")
 
     def _check_quant_grad_possible(self) -> None:
         if getattr(self, "_drop_packed", False) and self.indices.numel() == 0:
@@ -300,7 +316,9 @@ class VQuantLinear(nn.Module):
         drop_packed=True makes the module DECODE-ONLY: once the index lists exist the packed `indices` are freed
         (4.2 instead of 7.2 bytes per index resident).  Calls with more than one token, `dequant()` and saving the
         state_dict are no longer possible; reloading a checkpoint restores them.  `set_lists_prefill()` brings back
-        multi-token calls, `dequant()` and the input gradient, computed from the lists."""
+        multi-token calls, `dequant()` and the input gradient, computed from the lists.  A vector-length-16 layer can
+        be made decode-only when both `set_list_decode()` and `set_lists_prefill()` are on (4.25 instead of 7.25
+        bytes per index); otherwise it is refused before anything is freed."""
         if rebuild:
             if getattr(self, "_drop_packed", False) and self.indices.numel() == 0:
                 raise RuntimeError("prepare(rebuild=True): this VQuantLinear is decode-only (prepare(drop_packed="
@@ -326,6 +344,14 @@ class VQuantLinear(nn.Module):
                 self.indices.data = torch.empty(0, dtype=self.indices.dtype, device=self.indices.device)
             self._packed, self._drop_packed = None, True
         return self
+
+    def _save_to_state_dict(self, destination, prefix, keep_vars):
+        # a decode-only v = 16 module would save a checkpoint without its packed index words, which no module loads
+        if self.vector_len == 16 and self._decode_only():
+            raise RuntimeError("state_dict: this vector-length-16 VQuantLinear is decode-only (prepare(drop_packed="
+                               "True)); its packed index words were freed and cannot be saved; reload the checkpoint "
+                               "to get a module that can be saved")
+        super()._save_to_state_dict(destination, prefix, keep_vars)
 
     def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs):
         # a decode-only module (prepare(drop_packed=True)) freed its packed words: make room for the checkpoint's

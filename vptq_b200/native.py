@@ -265,7 +265,7 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
               perm: Optional[torch.Tensor], weight_scale: Optional[torch.Tensor],
               weight_bias: Optional[torch.Tensor], bias: Optional[torch.Tensor],
               derive: bool = True, lists: Optional[bool] = None, drop_packed: bool = False,
-              lists16: bool = False) -> LinearDesc:
+              lists16: bool = False, lists_prefill: bool = False) -> LinearDesc:
     """Describe one layer's tensors for the C ABI.  Tensors are borrowed: keep them alive.
 
     With `derive` (default) the load-time derivatives the ABI accepts are built here, once:
@@ -283,7 +283,10 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
 
     `drop_packed`: decode-only descriptor -- once the lists are built the descriptor forgets the packed words
     (`indices` = NULL), so the caller may free them: 4.2 instead of 7.2 bytes per index.  Multi-token calls,
-    dequant and prefill then return VPTQ_ERR_UNSUPPORTED.  Refused for layers without lists.
+    dequant and prefill then return VPTQ_ERR_UNSUPPORTED.  Refused for layers without lists.  A vector-length-16
+    layer (`lists16`) becomes decode-only only with `lists_prefill` (VQuantLinear.set_lists_prefill), whose routes
+    (include/vptq_b200_lists_dense.h) serve every call its list kernel does not: 4.25 instead of 7.25 bytes per
+    index.  Refused when its lists take no token count (lists16_max_tokens 0).
     """
     if indices.dtype != torch.int32:
         raise RuntimeError("`indices` must be packed int32 words (is_indice_packed=True); "
@@ -349,12 +352,14 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
         d.lists_stream, d.lists_tab, d.lists_tile_cols = stream.data_ptr(), tab.data_ptr(), int(tcw)
         d._keep = d._keep + (stream, tab)
     if drop_packed:
-        if d.vector_len != 8 and d.lists_stream:
-            raise RuntimeError("drop_packed: decode-only descriptors exist for vector_len 8 only (a vector-length-16 "
-                               "layer's lists serve single- and few-token decode, not prefill or dequant)")
-        if not d.lists_stream:
+        if d.vector_len != 8 and d.lists_stream and not lists_prefill:
+            raise RuntimeError("drop_packed: decode-only descriptors exist for vector_len 8 only, unless a "
+                               "vector-length-16 layer also opts in to prefill from its lists (set_lists_prefill): "
+                               "its list kernel serves single- and few-token decode, not prefill or dequant")
+        if not d.lists_stream or (d.vector_len == 16 and lists16_max_tokens(d) == 0):
             raise RuntimeError("drop_packed: this layer has no index lists (not eligible, its slices x column tiles "
-                               "exceed the device's SM count, or lists=False)")
+                               "exceed the device's SM count, lists=False, or for vector_len 16 no set_list_decode or "
+                               "lists its kernel takes at no token count)")
         d.indices = None
     return d
 

@@ -12,7 +12,8 @@ Function names, argument order and argument meaning are the reference's
   (`_lists_prefill`, VQuantLinear.set_lists_prefill): a decode-only descriptor takes every call the list kernels do
   not through the GEMM with the weight written from the index lists (include/vptq_b200_lists_dense.h), and its input
   gradient likewise.  Opt-in (`_list_decode`, VQuantLinear.set_list_decode): 1..lists16_max_tokens tokens of a
-  vector-length-16 layer with index lists -> the v = 16 list kernel (include/vptq_b200_lists16.h);
+  vector-length-16 layer with index lists -> the v = 16 list kernel (include/vptq_b200_lists16.h); with both
+  opt-ins such a layer may be decode-only too, and its other calls take the GEMM from the lists;
 * `argsort(perm)` is not recomputed on every call (the reference does, :208-211).
 """
 from __future__ import annotations
@@ -30,7 +31,7 @@ __all__ = ["dequant", "quant_gemm", "quant_gemv_v2"]
 def _desc(*, dtype, indices, centroids, outlier_indices, outlier_centroids, residual_centroids, perm,
           weight_scale, weight_bias, bias, vector_len, outlier_vector_len, num_codebooks, num_centroids,
           num_outlier_centroids, num_res_centroids, group_size, outlier_size, in_features, out_features,
-          derive=True, lists=None, drop_packed=False, lists16=False):
+          derive=True, lists=None, drop_packed=False, lists16=False, lists_prefill=False):
     if perm is not None and perm.dtype not in (torch.int16, torch.uint16):
         # unpacked checkpoints keep perm as int64 (vqlinear.py:191-196)
         perm = perm.to(torch.int64).to(torch.uint16).contiguous()
@@ -41,7 +42,8 @@ def _desc(*, dtype, indices, centroids, outlier_indices, outlier_centroids, resi
         outlier_vector_len=outlier_vector_len, num_outlier_centroids=num_outlier_centroids, indices=indices,
         centroids=centroids, res_centroids=residual_centroids, outlier_indices=outlier_indices,
         outlier_centroids=outlier_centroids, perm=perm, weight_scale=weight_scale, weight_bias=weight_bias,
-        bias=bias, derive=derive, lists=lists, drop_packed=drop_packed, lists16=lists16), perm
+        bias=bias, derive=derive, lists=lists, drop_packed=drop_packed, lists16=lists16,
+        lists_prefill=lists_prefill), perm
 
 
 def dequant(
@@ -196,7 +198,7 @@ def quant_gemm(
 
     `_list_decode` (VQuantLinear.set_list_decode): a kept descriptor of a vector-length-16 layer carries index lists,
     and 1..lists16_max_tokens tokens run the v = 16 list kernel (include/vptq_b200_lists16.h); every other call is
-    routed as without it."""
+    routed as without it.  With `_lists_prefill` too, `_drop_packed` may make that descriptor decode-only."""
     if vector_quant_dim == "in":
         raise ValueError("Not implemented yet.")
     if not is_indice_packed:
@@ -221,7 +223,7 @@ def quant_gemm(
             # a one-off descriptor (reference-style direct call) must not pay for re-bucketing the whole layer:
             # the slice x tile lists are built only when the caller keeps the descriptor (VQuantLinear does)
             lists=None if _desc_cache is not None else False, drop_packed=_drop_packed,
-            lists16=_list_decode and _desc_cache is not None)
+            lists16=_list_decode and _desc_cache is not None, lists_prefill=_lists_prefill)
         if _desc_cache is not None:
             _desc_cache.extend([desc, perm_])   # keep the converted perm alive with the descriptor
     x2d = x.reshape(-1, in_features)
@@ -255,9 +257,13 @@ def _forward(desc, x2d: torch.Tensor, out_features: int, batched: bool = False,
     y = torch.empty(tokens, out_features, dtype=x2d.dtype, device=x2d.device)
     if tokens == 0:
         return y
-    if list_decode and desc.vector_len == 16 and desc.lists_stream and x2d.data_ptr() % 16 == 0 and \
+    aligned = x2d.data_ptr() % 16 == 0
+    if list_decode and desc.vector_len == 16 and desc.lists_stream and (aligned or not desc.indices) and \
             tokens <= native.lists16_max_tokens(desc):
-        native.quant_gemv_lists16(desc, x2d, y)
+        # a decode-only descriptor has no other route for these calls: a misaligned x runs on an aligned copy (each
+        # token's outputs do not depend on where x lives)
+        xa = x2d if aligned else x2d.clone(memory_format=torch.contiguous_format)
+        native.quant_gemv_lists16(desc, xa, y)
     elif batched and tokens >= 2 and desc.lists_stream and x2d.data_ptr() % 16 == 0 and \
             tokens <= native.batch_max_tokens(desc):
         native.quant_gemv_batch(desc, x2d, y)
