@@ -223,62 +223,10 @@ def test_cutoff_partition_regimes():
 
 
 # ---------------------------------------------------------------- python routing with native stubbed
-class _Desc:
-    def __init__(self, lists=True):
-        self.lists_stream = 1 if lists else 0
-
-
-def _stub(monkeypatch, max_tokens=8):
-    from vptq_b200 import native
-    calls = []
-    monkeypatch.setattr(native, "quant_gemv", lambda d, x, y, flags=0: calls.append(("gemv", x.shape[0])))
-    monkeypatch.setattr(native, "quant_gemm", lambda d, x, y, flags=0: calls.append(("gemm", x.shape[0])))
-    monkeypatch.setattr(native, "quant_gemv_batch", lambda d, x, y, flags=0: calls.append(("batch", x.shape[0])))
-
-    def bmt(d):
-        calls.append(("max", None))
-        return max_tokens
-    monkeypatch.setattr(native, "batch_max_tokens", bmt)
-    return calls
-
-
-def _aligned(tokens, I=64):
-    buf = torch.zeros(tokens * I + 16, dtype=torch.float16)
-    off = (-buf.data_ptr() % 16) // 2
-    return buf[off:off + tokens * I].view(tokens, I)
-
-
-def test_opted_out_calls_never_reach_the_batched_entry_points(monkeypatch):
-    from vptq_b200 import ops
-    calls = _stub(monkeypatch)
-    for tokens in range(1, 12):
-        ops._forward(_Desc(), _aligned(tokens), 32)
-        ops._forward(_Desc(), _aligned(tokens), 32, False)
-    assert calls and all(c[0] in ("gemv", "gemm") for c in calls)
-    assert [c for c in calls if c[0] == "gemv"] == [("gemv", t) for t in (1, 1, 2, 2)]
-
-
-def test_opted_in_routing(monkeypatch):
-    from vptq_b200 import ops
-    calls = _stub(monkeypatch)
-    route = {}
-    for tokens in range(1, 12):
-        calls.clear()
-        ops._forward(_Desc(), _aligned(tokens), 32, True)
-        route[tokens] = [c[0] for c in calls if c[0] != "max"]
-    assert route == {1: ["gemv"], **{t: ["batch"] for t in range(2, 9)}, 9: ["gemm"], 10: ["gemm"], 11: ["gemm"]}
-    calls.clear()
-    ops._forward(_Desc(lists=False), _aligned(4), 32, True)       # no index lists: as without the opt-in
-    assert calls == [("gemm", 4)]
-    calls = _stub(monkeypatch, max_tokens=0)                      # not eligible
-    ops._forward(_Desc(), _aligned(2), 32, True)
-    assert [c for c in calls if c[0] != "max"] == [("gemv", 2)]
-
-
-def test_module_passes_the_flag(monkeypatch):
+def test_module_passes_the_batched_decode_opt_in(monkeypatch):
     from vptq_b200 import VQuantLinear, ops
     seen = []
-    monkeypatch.setattr(ops, "quant_gemm", lambda x, **kw: seen.append(kw["_batched_decode"]))
+    monkeypatch.setattr(ops, "quant_gemm", lambda x, **kw: seen.append(kw["_opt_ins"].batched_decode))
     m = VQuantLinear(64, 32, vector_lens=[-1, 8], num_centroids=[-1, 256], num_res_centroids=[-1, -1], group_num=1,
                      group_size=64, outlier_size=0, indices_as_float=False, is_indice_packed=True,
                      dtype=torch.float16, enable_proxy_error=False)
@@ -291,7 +239,7 @@ def test_module_passes_the_flag(monkeypatch):
     assert seen == [False, True, False]
 
 
-def test_set_batched_decode_reaches_fused_members():
+def test_set_batched_decode_reaches_every_fused_member():
     import vptq_b200
     from vptq_b200 import VQuantLinear
     from vptq_b200.fuse import FusedGroup, FusedMember
@@ -304,6 +252,6 @@ def test_set_batched_decode_reaches_fused_members():
     g = FusedGroup([a, b])
     model = torch.nn.Sequential(FusedMember(a, g, 0), FusedMember(b, g, 1), c)
     assert vptq_b200.set_batched_decode(model) == 3
-    assert a._batched_decode and b._batched_decode and c._batched_decode
+    assert a._opt_ins.batched_decode and b._opt_ins.batched_decode and c._opt_ins.batched_decode
     assert vptq_b200.set_batched_decode(model, False) == 3
-    assert not (a._batched_decode or b._batched_decode or c._batched_decode)
+    assert not (a._opt_ins.batched_decode or b._opt_ins.batched_decode or c._opt_ins.batched_decode)

@@ -181,75 +181,6 @@ def test_refusals_before_any_launch_v16():
         assert deq(ctypes.byref(d), 0x1000, 8192, 0, None) < 0
 
 
-# ---------------------------------------------------------------- python routing with native stubbed
-class _Desc:
-    def __init__(self, indices=0):
-        self.lists_stream = 1
-        self.vector_len = 16
-        self.indices = indices     # 0: decode-only
-
-
-def _stub(monkeypatch, max_tokens=4):
-    from vptq_b200 import native
-    calls = []
-
-    def rec(name):
-        return lambda d, x, y, flags=0: calls.append((name, x.shape[0], x.data_ptr() % 16, x.clone(), flags))
-    for name in ("quant_gemv", "quant_gemm", "quant_gemv_batch", "quant_gemv_lists16", "lists_quant_gemm",
-                 "quant_gemm_dgrad"):
-        monkeypatch.setattr(native, name, rec(name))
-    monkeypatch.setattr(native, "batch_max_tokens", lambda d: 0)   # v = 16: the batched kernel takes nothing
-    monkeypatch.setattr(native, "lists16_max_tokens", lambda d: max_tokens)
-    return calls
-
-
-def _rows(tokens, I=64, off=0):
-    buf = torch.arange(tokens * I + 32, dtype=torch.float16)
-    o = (-buf.data_ptr() % 16) // 2 + off
-    return buf[o:o + tokens * I].view(tokens, I)
-
-
-@pytest.mark.parametrize("batched", [False, True])
-def test_decode_only_v16_routes_only_to_list_entry_points(monkeypatch, batched):
-    from vptq_b200 import ops
-    for max_tokens in (4, 2, 1):
-        calls = _stub(monkeypatch, max_tokens)
-        for tokens in list(range(1, 10)) + [2048]:
-            for off in (0, 1):
-                calls.clear()
-                ops._forward(_Desc(), _rows(tokens, off=off), 32, batched, True, True)
-                want = "quant_gemv_lists16" if tokens <= max_tokens else "lists_quant_gemm"
-                assert [c[0] for c in calls] == [want], (max_tokens, tokens, off)
-                if want == "quant_gemv_lists16":     # a misaligned x runs on an aligned copy of the same values
-                    assert calls[0][2] == 0 and torch.equal(calls[0][3], _rows(tokens, off=off))
-
-
-def test_full_v16_module_keeps_todays_routes(monkeypatch):
-    """with the packed words, a misaligned x is still left to the generic kernel (no copy)"""
-    from vptq_b200 import ops
-    calls = _stub(monkeypatch)
-    ops._forward(_Desc(indices=1), _rows(1, off=1), 32, False, True, True)
-    assert [c[0] for c in calls] == ["quant_gemv"]
-    calls.clear()
-    ops._forward(_Desc(indices=1), _rows(9), 32, False, True, True)
-    assert [c[0] for c in calls] == ["quant_gemm"]
-
-
-def test_input_gradient_of_decode_only_v16_reads_the_lists(monkeypatch):
-    from vptq_b200 import native, ops
-    calls = _stub(monkeypatch)
-
-    class _Ctx:
-        lists_prefill = True
-        needs_input_grad = (True, True)
-    d = _Desc()
-    d.in_features = 64
-    dy = torch.ones(5, 32, dtype=torch.float16)
-    dx, db = ops._input_grads(_Ctx(), d, dy)
-    assert [(c[0], c[4]) for c in calls] == [("lists_quant_gemm", native.FLAG_TRANSPOSE)]
-    assert dx.shape == (5, 64) and torch.equal(db, torch.full((32,), 5.0, dtype=torch.float16))
-
-
 # ---------------------------------------------------------------- prepare(drop_packed=True) refusal matrix
 def _cpu_make_desc(monkeypatch, max_tokens=4, built=True):
     """native.make_desc on CPU tensors: the builder, the SM count and the token limit stubbed"""
@@ -325,13 +256,13 @@ def test_module_hands_both_opt_ins_to_the_descriptor_and_keeps_indices_on_refusa
     assert not m._decode_only()
 
 
-def test_decode_only_v16_module_keeps_its_opt_ins():
+def test_decode_only_v16_module_keeps_both_list_opt_ins():
     m = _lin().set_list_decode().set_lists_prefill()
     m._drop_packed, m.indices.data = True, torch.empty(0, dtype=torch.int32)   # as prepare(drop_packed=True) leaves it
     for off in (m.set_list_decode, m.set_lists_prefill):
         with pytest.raises(RuntimeError, match="decode-only"):
             off(False)
-    assert m._list_decode and m._lists_prefill
+    assert m._opt_ins.list_decode and m._opt_ins.lists_prefill
     assert m.set_list_decode(True) is m and m.set_lists_prefill(True) is m   # turning them on again is harmless
     with pytest.raises(RuntimeError, match="decode-only"):
         m.set_quant_grad(True)

@@ -371,55 +371,6 @@ def test_partition_does_not_depend_on_the_token_count():
 
 
 # ---------------------------------------------------------------- python routing with native stubbed
-class _Desc:
-    def __init__(self, v=16, lists=True):
-        self.lists_stream = 1 if lists else 0
-        self.vector_len = v
-        self.indices = 1
-
-
-def _stub(monkeypatch, max_tokens=4):
-    from vptq_b200 import native
-    calls = []
-    monkeypatch.setattr(native, "quant_gemv", lambda d, x, y, flags=0: calls.append(("gemv", x.shape[0])))
-    monkeypatch.setattr(native, "quant_gemm", lambda d, x, y, flags=0: calls.append(("gemm", x.shape[0])))
-    monkeypatch.setattr(native, "quant_gemv_batch", lambda d, x, y, flags=0: calls.append(("batch", x.shape[0])))
-    monkeypatch.setattr(native, "quant_gemv_lists16", lambda d, x, y, flags=0: calls.append(("l16", x.shape[0])))
-    monkeypatch.setattr(native, "batch_max_tokens", lambda d: 8)
-    monkeypatch.setattr(native, "lists16_max_tokens", lambda d: max_tokens)
-    return calls
-
-
-def _aligned(tokens, I=64, off=0):
-    buf = torch.zeros(tokens * I + 32, dtype=torch.float16)
-    o = (-buf.data_ptr() % 16) // 2 + off
-    return buf[o:o + tokens * I].view(tokens, I)
-
-
-def test_routing(monkeypatch):
-    from vptq_b200 import ops
-    calls = _stub(monkeypatch)
-    route = {}
-    for tokens in range(1, 8):
-        calls.clear()
-        ops._forward(_Desc(), _aligned(tokens), 32, False, False, True)
-        route[tokens] = [c[0] for c in calls]
-    assert route == {**{t: ["l16"] for t in range(1, 5)}, 5: ["gemm"], 6: ["gemm"], 7: ["gemm"]}
-    for desc, x, opt in ((_Desc(), _aligned(2), False),          # not opted in
-                         (_Desc(lists=False), _aligned(2), True),  # no lists (ineligible layer)
-                         (_Desc(v=8), _aligned(2), True),          # a v = 8 layer
-                         (_Desc(), _aligned(2, off=1), True)):     # x not 16-byte aligned
-        calls.clear()
-        ops._forward(desc, x, 32, False, False, opt)
-        assert calls == [("gemv", 2)]
-    calls = _stub(monkeypatch, max_tokens=0)                       # the kernel refuses these layers
-    ops._forward(_Desc(), _aligned(1), 32, False, False, True)
-    assert calls == [("gemv", 1)]
-    calls = _stub(monkeypatch, max_tokens=2)
-    ops._forward(_Desc(), _aligned(3), 32, False, False, True)
-    assert calls == [("gemm", 3)]
-
-
 def _lin(v=16, I=64):
     from vptq_b200 import VQuantLinear
     return VQuantLinear(I, 32, vector_lens=[-1, v], num_centroids=[-1, 256], num_res_centroids=[-1, -1], group_num=1,
@@ -427,10 +378,10 @@ def _lin(v=16, I=64):
                         dtype=torch.float16, enable_proxy_error=False)
 
 
-def test_module_passes_the_flag_and_drops_a_descriptor_without_lists(monkeypatch):
+def test_module_passes_the_list_decode_opt_in_and_drops_a_descriptor_without_lists(monkeypatch):
     from vptq_b200 import ops
     seen = []
-    monkeypatch.setattr(ops, "quant_gemm", lambda x, **kw: seen.append(kw["_list_decode"]))
+    monkeypatch.setattr(ops, "quant_gemm", lambda x, **kw: seen.append(kw["_opt_ins"].list_decode))
     m = _lin()
     x = torch.zeros(2, 64, dtype=torch.float16)
     m(x)
@@ -449,16 +400,16 @@ def test_module_passes_the_flag_and_drops_a_descriptor_without_lists(monkeypatch
         assert (m._desc_cache == []) == dropped and (m._desc_key is None) == dropped, v
 
 
-def test_set_list_decode_reaches_fused_members_and_fuse_takes_v16_groups():
+def test_set_list_decode_reaches_every_fused_member_and_fuse_takes_v16_groups():
     import vptq_b200
     from vptq_b200.fuse import FusedGroup, FusedMember, _eligible
     a, b, c = _lin(), _lin(), _lin()
     g = FusedGroup([a, b])
     model = torch.nn.Sequential(FusedMember(a, g, 0), FusedMember(b, g, 1), c)
     assert vptq_b200.set_list_decode(model) == 3
-    assert a._list_decode and b._list_decode and c._list_decode
+    assert a._opt_ins.list_decode and b._opt_ins.list_decode and c._opt_ins.list_decode
     assert vptq_b200.set_list_decode(model, False) == 3
-    assert not (a._list_decode or b._list_decode or c._list_decode)
+    assert not (a._opt_ins.list_decode or b._opt_ins.list_decode or c._opt_ins.list_decode)
     assert _eligible([_lin(16), _lin(16)]) and _eligible([_lin(8), _lin(8)])
     assert not _eligible([_lin(16), _lin(8)]) and not _eligible([_lin(4), _lin(4)])
 

@@ -17,17 +17,11 @@ a member called alone, an activation that changed in between -- takes the member
 are those of the unfused model in every case.  `fuse` also builds every layer's descriptor and load-time
 index lists (`VQuantLinear.prepare`), so nothing is allocated or re-bucketed inside the first forward.
 
-After `set_batched_decode(model)` a group whose members all opted in also launches 2..8-token activations as one
-batched list-kernel launch (include/vptq_b200_batch.h), with the same results as its members' own forwards.
-
-After `set_list_decode(model)` a group of vector-length-16 layers that all opted in launches 1..4-token activations
-as one launch of the v = 16 list kernel (include/vptq_b200_lists16.h).  Without it such a group is never fused: each
-member takes its own forward.
-
-`set_lists_prefill(model)` lets decode-only layers (`prepare(drop_packed=True)`) serve prompts from their index lists
-(include/vptq_b200_lists_dense.h).  The generic fused launch cannot take 2-token calls of such a group, so those go to
-each member's own forward.  A decode-only vector-length-16 group (set_list_decode too) only ever launches the v = 16
-list kernel; every call it declines goes to each member's own forward, which never needs the packed words either.
+Which calls a group launches as one is decided by `ops.route`, the same function that routes a single layer's calls:
+1..2-token calls through the generic fused GEMV; with every member opted in (`set_batched_decode(model)`,
+`set_list_decode(model)`) the batched list kernel (include/vptq_b200_batch.h) or, for vector-length-16 groups, the
+v = 16 list kernel (include/vptq_b200_lists16.h).  Every other call -- among them those a decode-only member serves
+from its index lists (`set_lists_prefill(model)`) -- goes to each member's own forward, with the same results.
 """
 from __future__ import annotations
 
@@ -36,7 +30,7 @@ from typing import Dict, Iterable, List, Optional, Sequence, Tuple
 import torch
 import torch.nn as nn
 
-from . import native
+from . import native, ops
 from .layers import VQuantLinear
 
 __all__ = ["fuse", "unfuse", "set_quant_grad", "set_batched_decode", "set_lists_prefill", "set_list_decode", "FusedGroup",
@@ -79,7 +73,8 @@ class FusedGroup:
         return [l._desc_cache[0] for l in self.layers]
 
     def outputs(self, x: torch.Tensor, index: int) -> Optional[torch.Tensor]:
-        """[tokens, sum(widths)] for a decode activation, None when this call must not be fused.
+        """[tokens, sum(widths)] when the group launches this call as one (`ops.route`), None when each member must run
+        its own forward.
 
         The cached outputs are handed to every member at most once: an address + version match alone could be a
         NEW tensor the caching allocator placed where the previous activation lived."""
@@ -87,17 +82,7 @@ class FusedGroup:
             return None           # the member's own forward records the autograd graph (same values)
         x2 = x.reshape(-1, x.shape[-1])
         tokens = x2.shape[0]
-        if not x.is_cuda or tokens < 1 or x2.stride(-1) != 1 or (tokens > 1 and x2.stride(0) < x2.shape[1]):
-            return None
-        if self.layers[0].vector_len == 16:
-            return self._outputs16(x, x2, index)
-        # 2..8 tokens: the batched list kernel when every member opted in (set_batched_decode) and it takes them
-        batched = tokens >= 2 and all(getattr(l, "_batched_decode", False) for l in self.layers)
-        if tokens > 2 and not batched:
-            return None
-        # decode-only members (set_lists_prefill) route 2-token calls the batched kernel does not take themselves
-        lists_member = tokens == 2 and any(getattr(l, "_lists_prefill", False) and l._decode_only() for l in self.layers)
-        if lists_member and not batched:
+        if not x.is_cuda or x2.stride(-1) != 1 or (tokens > 1 and x2.stride(0) < x2.shape[1]):
             return None
         key = activation_key(x)
         if key == self._key and self._out is not None and not (self._served >> index) & 1:
@@ -105,46 +90,24 @@ class FusedGroup:
             if self._served == (1 << len(self.layers)) - 1:
                 self._key = None
             return self._out
-        descs = self._descs(x)
-        if batched and (x2.data_ptr() % 16 or tokens > native.batch_max_tokens(descs)):
-            if tokens > 2 or lists_member:
-                return None       # each member routes its own call (its own batched launch where it is eligible)
-            batched = False
-        fkey = tuple(id(d) for d in descs) + (tokens, batched)
-        if self._fused is None or fkey != self._fused_key:
-            self._out = torch.empty(tokens, sum(self.widths), dtype=x.dtype, device=x.device)
-            offs = [0]
-            for w in self.widths:
-                offs.append(offs[-1] + w)
-            fused = native.FusedGemvBatch if batched else native.FusedGemv
-            self._fused = fused(descs, [self._out[:, a:b] for a, b in zip(offs[:-1], offs[1:])])
-            self._fused_key = fkey
-        self._fused(x2, self.flags)
-        self._key, self._served = key, 1 << index
-        return self._out
+        descs = []                # fetched once, by whichever of route() and the launch below needs them first
 
-    def _outputs16(self, x: torch.Tensor, x2: torch.Tensor, index: int) -> Optional[torch.Tensor]:
-        """outputs() of a vector-length-16 group: one launch of the v = 16 list kernel when every member opted in
-        (set_list_decode) and it takes the whole group at this token count, else None (each member's own forward)."""
-        if not all(getattr(l, "_list_decode", False) for l in self.layers):
+        def fetch():
+            if not descs:
+                descs.extend(self._descs(x))
+            return descs
+        r = ops.route(fetch, tokens, x2.data_ptr() % 16 == 0, [l._opt_ins for l in self.layers],
+                      self.layers[0].vector_len)
+        if r is None:
             return None
-        tokens = x2.shape[0]
-        key = activation_key(x)
-        if key == self._key and self._out is not None and not (self._served >> index) & 1:
-            self._served |= 1 << index
-            if self._served == (1 << len(self.layers)) - 1:
-                self._key = None
-            return self._out
-        descs = self._descs(x)
-        if x2.data_ptr() % 16 or tokens > native.lists16_max_tokens(descs):
-            return None
-        fkey = tuple(id(d) for d in descs) + (tokens, "lists16")
+        fkey = tuple(id(d) for d in fetch()) + (tokens, r)
         if self._fused is None or fkey != self._fused_key:
             self._out = torch.empty(tokens, sum(self.widths), dtype=x.dtype, device=x.device)
             offs = [0]
             for w in self.widths:
                 offs.append(offs[-1] + w)
-            self._fused = native.FusedGemvLists16(descs, [self._out[:, a:b] for a, b in zip(offs[:-1], offs[1:])])
+            fused = {ops.GEMV: native.FusedGemv, ops.BATCH: native.FusedGemvBatch, ops.LISTS16: native.FusedGemvLists16}
+            self._fused = fused[r](descs, [self._out[:, a:b] for a, b in zip(offs[:-1], offs[1:])])
             self._fused_key = fkey
         self._fused(x2, self.flags)
         self._key, self._served = key, 1 << index
@@ -238,11 +201,16 @@ def fuse(model: nn.Module, groups: Sequence[Sequence[str]] = DEFAULT_GROUPS, pdl
     return made
 
 
+def _layers(model: nn.Module) -> List[VQuantLinear]:
+    """Every VQuantLinear of `model`, fused members included."""
+    layers = [mod.layer if isinstance(mod, FusedMember) else mod for mod in model.modules()]
+    return [l for l in layers if isinstance(l, VQuantLinear)]
+
+
 def set_quant_grad(model: nn.Module, enabled: bool = True) -> int:
     """`VQuantLinear.set_quant_grad(enabled)` on every VQuantLinear of `model`, fused members included.  Returns how
     many layers it reached."""
-    layers = [mod.layer if isinstance(mod, FusedMember) else mod for mod in model.modules()]
-    layers = [l for l in layers if isinstance(l, VQuantLinear)]
+    layers = _layers(model)
     if enabled:
         for l in layers:          # refuse before any layer changes: all or nothing
             l._check_quant_grad_possible()
@@ -254,18 +222,16 @@ def set_quant_grad(model: nn.Module, enabled: bool = True) -> int:
 def set_batched_decode(model: nn.Module, enabled: bool = True) -> int:
     """`VQuantLinear.set_batched_decode(enabled)` on every VQuantLinear of `model`, fused members included.  Returns
     how many layers it reached."""
-    layers = [mod.layer if isinstance(mod, FusedMember) else mod for mod in model.modules()]
-    layers = [l for l in layers if isinstance(l, VQuantLinear)]
+    layers = _layers(model)
     for l in layers:
         l.set_batched_decode(enabled)
     return len(layers)
 
 
 def set_lists_prefill(model: nn.Module, enabled: bool = True) -> int:
-    """`VQuantLinear.set_lists_prefill(enabled)` on every VQuantLinear of `model`, fused members included.  Returns
-    how many layers it reached."""
-    layers = [mod.layer if isinstance(mod, FusedMember) else mod for mod in model.modules()]
-    layers = [l for l in layers if isinstance(l, VQuantLinear)]
+    """`VQuantLinear.set_lists_prefill(enabled)` on every VQuantLinear of `model`, fused members included.  Returns how
+    many layers it reached."""
+    layers = _layers(model)
     for l in layers:
         l.set_lists_prefill(enabled)
     return len(layers)
@@ -274,8 +240,7 @@ def set_lists_prefill(model: nn.Module, enabled: bool = True) -> int:
 def set_list_decode(model: nn.Module, enabled: bool = True) -> int:
     """`VQuantLinear.set_list_decode(enabled)` on every VQuantLinear of `model`, fused members included (it changes
     only vector-length-16 layers the v = 16 list kernel takes).  Returns how many layers it reached."""
-    layers = [mod.layer if isinstance(mod, FusedMember) else mod for mod in model.modules()]
-    layers = [l for l in layers if isinstance(l, VQuantLinear)]
+    layers = _layers(model)
     for l in layers:
         l.set_list_decode(enabled)
     return len(layers)

@@ -163,9 +163,9 @@ class VQuantLinear(nn.Module):
         self._desc_key = None
         self._packed = None              # lazily packed indices for unpacked checkpoints
         self._quant_grad = False         # set_quant_grad
-        self._batched_decode = False     # set_batched_decode
-        self._lists_prefill = False      # set_lists_prefill
-        self._list_decode = False        # set_list_decode
+        self._opt_ins = ops.NO_OPT_INS   # set_batched_decode, set_lists_prefill, set_list_decode
+        self._drop_packed = False        # prepare(drop_packed=True) freed the packed index words
+        self._drop_request = False       # inside prepare(drop_packed=True): build a decode-only descriptor
 
     # ------------------------------------------------------------------------------------------
     def _tensors(self):
@@ -233,7 +233,7 @@ class VQuantLinear(nn.Module):
         index lists) are routed as without the opt-in.  Its results may differ from the default routes in the low-order
         bits; each token's outputs do not depend on the other tokens of the call.  A decode-only module
         (`prepare(drop_packed=True)`) with the opt-in serves 2..8 tokens."""
-        self._batched_decode = bool(enabled)
+        self._opt_ins = self._opt_ins._replace(batched_decode=bool(enabled))
         return self
 
     def set_lists_prefill(self, enabled: bool = True) -> "VQuantLinear":
@@ -252,7 +252,7 @@ class VQuantLinear(nn.Module):
         state_dict (the checkpoint would lack the packed words)."""
         if not enabled:
             self._check_v16_opt_ins_kept("set_lists_prefill(False)")
-        self._lists_prefill = bool(enabled)
+        self._opt_ins = self._opt_ins._replace(lists_prefill=bool(enabled))
         return self
 
     def set_list_decode(self, enabled: bool = True) -> "VQuantLinear":
@@ -272,14 +272,14 @@ class VQuantLinear(nn.Module):
         enabled = bool(enabled)
         if not enabled:
             self._check_v16_opt_ins_kept("set_list_decode(False)")
-        if enabled and not self._list_decode and self.vector_len == 16 and self._desc_cache and \
+        if enabled and not self._opt_ins.list_decode and self.vector_len == 16 and self._desc_cache and \
                 not self._desc_cache[0].lists_stream:
             self._desc_cache, self._desc_key = [], None
-        self._list_decode = enabled
+        self._opt_ins = self._opt_ins._replace(list_decode=enabled)
         return self
 
     def _decode_only(self) -> bool:
-        return getattr(self, "_drop_packed", False) and self.indices.numel() == 0
+        return self._drop_packed and self.indices.numel() == 0
 
     def _check_v16_opt_ins_kept(self, what: str) -> None:
         # a decode-only v = 16 module has no route for its calls without both list opt-ins
@@ -288,13 +288,13 @@ class VQuantLinear(nn.Module):
                                "and serves its calls from its index lists only; reload the checkpoint first")
 
     def _check_quant_grad_possible(self) -> None:
-        if getattr(self, "_drop_packed", False) and self.indices.numel() == 0:
+        if self._decode_only():
             raise RuntimeError("set_quant_grad: this VQuantLinear is decode-only (prepare(drop_packed=True)); the "
                                "packed index words the weight gradients need were freed; reload the checkpoint")
 
     def _quant_grad_needed(self) -> bool:
         """Opted in and some quantizer tensor requires grad: a forward under grad mode records a node."""
-        if not getattr(self, "_quant_grad", False):
+        if not self._quant_grad:
             return False
         _, cent, resc, _, outc, _, ws, wb, _ = self._tensors()
         return any(t is not None and t.requires_grad for t in (cent, resc, outc, ws, wb))
@@ -320,7 +320,7 @@ class VQuantLinear(nn.Module):
         be made decode-only when both `set_list_decode()` and `set_lists_prefill()` are on (4.25 instead of 7.25
         bytes per index); otherwise it is refused before anything is freed."""
         if rebuild:
-            if getattr(self, "_drop_packed", False) and self.indices.numel() == 0:
+            if self._decode_only():
                 raise RuntimeError("prepare(rebuild=True): this VQuantLinear is decode-only (prepare(drop_packed="
                                    "True)); its index lists cannot be rebuilt without the packed index words, which "
                                    "were freed; reload the checkpoint")
@@ -330,7 +330,7 @@ class VQuantLinear(nn.Module):
         if drop_packed:
             if not self.is_indice_packed:
                 raise RuntimeError("drop_packed needs a packed checkpoint (is_indice_packed=True)")
-            if getattr(self, "_quant_grad", False):
+            if self._quant_grad:
                 raise RuntimeError("prepare(drop_packed=True) on a module with set_quant_grad(True): the weight "
                                    "gradients need the packed index words; call set_quant_grad(False) first")
             self._desc_cache, self._desc_key = [], None
@@ -381,11 +381,10 @@ class VQuantLinear(nn.Module):
             return self.proxy_error_forward(W, H)   # quantizer-side debugging aid
         t = self._tensors()
         key = self._cache_key(t, x.dtype, x.device)
-        if getattr(self, "_drop_packed", False):
-            if self.indices.numel() == 0 and self._desc_cache:
-                key = self._desc_key                  # decode-only: the descriptor no longer depends on `indices`
-            else:
-                self._drop_packed = False             # a checkpoint was loaded again: a full module once more
+        if self._decode_only() and self._desc_cache:
+            key = self._desc_key                      # decode-only: the descriptor no longer depends on `indices`
+        elif self._drop_packed:
+            self._drop_packed = False                 # a checkpoint was loaded again: a full module once more
         if key != self._desc_key:                    # parameters were moved / reloaded / updated in place
             if not self._refresh_in_place(key):
                 self._desc_cache = []
@@ -401,15 +400,12 @@ class VQuantLinear(nn.Module):
             outlier_size=self.outlier_size, in_features=self.in_features, out_features=self.out_features,
             padding=self.padding, outlier_padding=self.outlier_padding,
             vector_quant_dim=self.vector_quant_dim, _desc_cache=self._desc_cache,
-            _drop_packed=getattr(self, "_drop_request", False), _quant_grad=getattr(self, "_quant_grad", False),
-            _batched_decode=getattr(self, "_batched_decode", False),
-            _lists_prefill=getattr(self, "_lists_prefill", False),
-            _list_decode=getattr(self, "_list_decode", False))
+            _drop_packed=self._drop_request, _quant_grad=self._quant_grad, _opt_ins=self._opt_ins)
 
     def dequant(self) -> torch.Tensor:
         """Dense [out_features, in_features] weight through the CUDA dequant kernel (from the index lists on a
         decode-only module with `set_lists_prefill()`)."""
-        if self._decode_only() and getattr(self, "_lists_prefill", False) and self._desc_cache:
+        if self._decode_only() and self._opt_ins.lists_prefill and self._desc_cache:
             cent = self.centroids.weight
             return native.lists_dense_weight(self._desc_cache[0], cent.dtype, cent.device)
         if self._decode_only():
@@ -425,7 +421,7 @@ class VQuantLinear(nn.Module):
             padding=self.padding, outlier_padding=self.outlier_padding, num_codebooks=self.num_codebooks,
             group_size=self.group_size, outlier_size=self.outlier_size, vector_len=self.vector_len,
             outlier_vector_len=self.outlier_vector_len, vector_quant_dim=self.vector_quant_dim,
-            _quant_grad=getattr(self, "_quant_grad", False))
+            _quant_grad=self._quant_grad)
 
     def proxy_error_forward(self, W, H):
         """diff^T diff * H with diff = dequant() - W (the quantizer's layer-wise proxy loss)."""

@@ -104,6 +104,18 @@ class LinearGrads(ctypes.Structure):
 
 GRAD_FIELDS = ("centroids", "res_centroids", "outlier_centroids", "weight_scale", "weight_bias")
 
+# (header, exports, version function, expected version, what it numbers), checked when the library loads; the
+# functions return int (ctypes' default restype) unless lib() says otherwise
+_INTERFACES = (
+    ("vptq_b200.h", EXPORTS, "vptq_b200_abi_version", ABI_VERSION, "ABI"),
+    ("vptq_b200_graph.h", GRAPH_EXPORTS, None, None, None),
+    ("vptq_b200_grad.h", GRAD_EXPORTS, "vptq_b200_grad_version", GRAD_VERSION, "grad interface"),
+    ("vptq_b200_batch.h", BATCH_EXPORTS, "vptq_b200_batch_version", BATCH_VERSION, "batch interface"),
+    ("vptq_b200_lists_dense.h", LISTS_DENSE_EXPORTS, "vptq_b200_lists_dense_version", LISTS_DENSE_VERSION,
+     "lists-dense interface"),
+    ("vptq_b200_lists16.h", LISTS16_EXPORTS, "vptq_b200_lists16_version", LISTS16_VERSION, "lists16 interface"),
+)
+
 _lib = None
 _lock = threading.Lock()
 
@@ -121,7 +133,12 @@ def lib() -> ctypes.CDLL:
                 f"{LIB_PATH} not found: build it with `python -m vptq_b200.build` "
                 "(vptq_b200 has no CPU or torch fallback)")
         L = ctypes.CDLL(LIB_PATH)
-        L.vptq_b200_abi_version.restype = ctypes.c_int
+        for header, exports, version, expected, what in _INTERFACES:
+            for f in exports:
+                if not hasattr(L, f):
+                    raise RuntimeError(f"{LIB_PATH} lacks {f} (include/{header}): rebuild it")
+            if version and getattr(L, version)() != expected:
+                raise RuntimeError(f"libvptq_b200.so {what} {getattr(L, version)()} != expected {expected}")
         L.vptq_b200_last_error.restype = ctypes.c_char_p
         L.vptq_b200_workspace_bytes.restype = ctypes.c_size_t
         L.vptq_b200_workspace_bytes.argtypes = [ctypes.POINTER(LinearDesc), ctypes.c_int32, ctypes.c_int32]
@@ -135,83 +152,33 @@ def lib() -> ctypes.CDLL:
         L.vptq_b200_linear_host.argtypes = [dp, vp, vp, i32, vp, vp, vp, sz, u32, vp]
         L.vptq_b200_quant_gemv_multi.argtypes = [i32, ctypes.POINTER(dp), vp, i64, ctypes.POINTER(vp),
                                                  ctypes.POINTER(i64), i32, u32, vp]
-        L.vptq_b200_quant_gemv_multi.restype = ctypes.c_int
         L.vptq_b200_quant_gemv_multi_ws.argtypes = [i32, ctypes.POINTER(dp), vp, i64, ctypes.POINTER(vp),
                                                     ctypes.POINTER(i64), i32, vp, sz, u32, vp]
-        L.vptq_b200_quant_gemv_multi_ws.restype = ctypes.c_int
         L.vptq_b200_quant_gemv_multi_tp.argtypes = [i32, ctypes.POINTER(dp), vp, i64, ctypes.POINTER(vp),
                                                     ctypes.POINTER(i64), i32, ctypes.POINTER(TpExchange), vp, sz, u32, vp]
-        L.vptq_b200_quant_gemv_multi_tp.restype = ctypes.c_int
         L.vptq_b200_lists_build_host.argtypes = [vp, i64, i32, i32, i32, i32, vp, vp, sz, vp, ctypes.POINTER(sz),
                                                  ctypes.POINTER(i32)]
-        L.vptq_b200_lists_build_host.restype = ctypes.c_int
         L.vptq_b200_lists_deal_host.argtypes = [vp, vp, i64, i32]
-        L.vptq_b200_lists_deal_host.restype = ctypes.c_int
         L.vptq_b200_tp_untag.argtypes = [vp, vp, i32, ctypes.POINTER(TpExchange), vp]
-        L.vptq_b200_tp_untag.restype = ctypes.c_int
         L.vptq_b200_debug_phase_stamps.argtypes = [vp]
         L.vptq_b200_debug_phase_stamps.restype = None
-        for f in GRAPH_EXPORTS:
-            if not hasattr(L, f):
-                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_graph.h): rebuild it")
         L.vptq_b200_stream_capture_id.argtypes = [vp, ctypes.POINTER(ctypes.c_uint64)]
-        L.vptq_b200_stream_capture_id.restype = ctypes.c_int
-        for f in ("vptq_b200_quant_gemv", "vptq_b200_quant_gemm", "vptq_b200_dequant", "vptq_b200_quant_gemv_v2",
-                  "vptq_b200_linear_host"):
-            getattr(L, f).restype = ctypes.c_int
-        if L.vptq_b200_abi_version() != ABI_VERSION:
-            raise RuntimeError(f"libvptq_b200.so ABI {L.vptq_b200_abi_version()} != expected {ABI_VERSION}")
-        for f in GRAD_EXPORTS:
-            if not hasattr(L, f):
-                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_grad.h): rebuild it")
         gp = ctypes.POINTER(LinearGrads)
-        L.vptq_b200_grad_version.restype = ctypes.c_int
         L.vptq_b200_grad_workspace_bytes.restype = ctypes.c_size_t
         L.vptq_b200_grad_workspace_bytes.argtypes = [dp, i32, i32]
         L.vptq_b200_quant_gemm_wgrad.argtypes = [dp, vp, i64, vp, i64, i32, gp, vp, sz, u32, vp]
-        L.vptq_b200_quant_gemm_wgrad.restype = ctypes.c_int
         L.vptq_b200_dequant_backward.argtypes = [dp, vp, i64, gp, vp, sz, u32, vp]
-        L.vptq_b200_dequant_backward.restype = ctypes.c_int
-        if L.vptq_b200_grad_version() != GRAD_VERSION:
-            raise RuntimeError(f"libvptq_b200.so grad interface {L.vptq_b200_grad_version()} != expected {GRAD_VERSION}")
-        for f in BATCH_EXPORTS:
-            if not hasattr(L, f):
-                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_batch.h): rebuild it")
-        L.vptq_b200_batch_version.restype = ctypes.c_int
         L.vptq_b200_quant_gemv_batch_max_tokens.argtypes = [i32, ctypes.POINTER(dp)]
-        L.vptq_b200_quant_gemv_batch_max_tokens.restype = ctypes.c_int
         L.vptq_b200_quant_gemv_batch.argtypes = [i32, ctypes.POINTER(dp), vp, i64, ctypes.POINTER(vp), ctypes.POINTER(i64),
                                                  i32, vp, sz, u32, vp]
-        L.vptq_b200_quant_gemv_batch.restype = ctypes.c_int
-        if L.vptq_b200_batch_version() != BATCH_VERSION:
-            raise RuntimeError(f"libvptq_b200.so batch interface {L.vptq_b200_batch_version()} != expected {BATCH_VERSION}")
-        for f in LISTS_DENSE_EXPORTS:
-            if not hasattr(L, f):
-                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_lists_dense.h): rebuild it")
-        L.vptq_b200_lists_dense_version.restype = ctypes.c_int
         L.vptq_b200_lists_dense_workspace_bytes.argtypes = [dp, i32, u32]
         L.vptq_b200_lists_dense_workspace_bytes.restype = ctypes.c_size_t
         L.vptq_b200_lists_dequant.argtypes = [dp, vp, i64, u32, vp]
-        L.vptq_b200_lists_dequant.restype = ctypes.c_int
         L.vptq_b200_lists_quant_gemm.argtypes = [dp, vp, i64, vp, i64, i32, vp, sz, u32, vp]
-        L.vptq_b200_lists_quant_gemm.restype = ctypes.c_int
-        if L.vptq_b200_lists_dense_version() != LISTS_DENSE_VERSION:
-            raise RuntimeError(f"libvptq_b200.so lists-dense interface {L.vptq_b200_lists_dense_version()} != expected "
-                               f"{LISTS_DENSE_VERSION}")
-        for f in LISTS16_EXPORTS:
-            if not hasattr(L, f):
-                raise RuntimeError(f"{LIB_PATH} lacks {f} (include/vptq_b200_lists16.h): rebuild it")
-        L.vptq_b200_lists16_version.restype = ctypes.c_int
         L.vptq_b200_quant_gemv_lists16_max_tokens.argtypes = [i32, ctypes.POINTER(dp)]
-        L.vptq_b200_quant_gemv_lists16_max_tokens.restype = ctypes.c_int
         L.vptq_b200_quant_gemv_lists16.argtypes = [i32, ctypes.POINTER(dp), vp, i64, ctypes.POINTER(vp),
                                                    ctypes.POINTER(i64), i32, vp, sz, u32, vp]
-        L.vptq_b200_quant_gemv_lists16.restype = ctypes.c_int
         L.vptq_b200_lists16_build_host.argtypes = L.vptq_b200_lists_build_host.argtypes
-        L.vptq_b200_lists16_build_host.restype = ctypes.c_int
-        if L.vptq_b200_lists16_version() != LISTS16_VERSION:
-            raise RuntimeError(f"libvptq_b200.so lists16 interface {L.vptq_b200_lists16_version()} != expected "
-                               f"{LISTS16_VERSION}")
         _lib = L
     return _lib
 
@@ -330,25 +297,17 @@ def make_desc(*, dtype: torch.dtype, in_features: int, out_features: int, vector
         d._keep = (ws_q, wb_q)
     if lists is None:
         lists = os.environ.get("VPTQ_B200_LISTS", LISTS_DEFAULT) != "0"
-    if lists and derive and _lists.eligible(
-            vector_len=d.vector_len, num_centroids=d.num_centroids, num_res_centroids=d.num_res_centroids,
-            num_codebooks=d.num_codebooks, outlier_size=d.outlier_size, in_features=d.in_features) and (
-            weight_scale is None or (weight_scale.data_ptr() % 16 == 0 and weight_bias.data_ptr() % 16 == 0)) and (
-            _lists.launchable(d.in_features, d.num_centroids, _sm_count(indices.device))):
-        stream, tab, tcw = _lists.build_lists(indices, num_centroids=d.num_centroids,
-                                              num_res_centroids=d.num_res_centroids, in_features=d.in_features,
-                                              out_features=d.out_features, perm=perm)
-        d.lists_stream, d.lists_tab, d.lists_tile_cols = stream.data_ptr(), tab.data_ptr(), int(tcw)
-        d._keep = d._keep + (stream, tab)
-    if lists16 and derive and d.vector_len == 16 and _lists.eligible(
+    # a vector-length-16 layer gets lists with index rows of 16 outputs, and only with `lists16`
+    list_vector_len = 16 if d.vector_len == 16 else 8
+    if (lists16 if list_vector_len == 16 else lists) and derive and _lists.eligible(
             vector_len=d.vector_len, num_centroids=d.num_centroids, num_res_centroids=d.num_res_centroids,
             num_codebooks=d.num_codebooks, outlier_size=d.outlier_size, in_features=d.in_features,
-            list_vector_len=16) and (
+            list_vector_len=list_vector_len) and (
             weight_scale is None or (weight_scale.data_ptr() % 16 == 0 and weight_bias.data_ptr() % 16 == 0)) and (
             _lists.launchable(d.in_features, d.num_centroids, _sm_count(indices.device))):
         stream, tab, tcw = _lists.build_lists(indices, num_centroids=d.num_centroids,
                                               num_res_centroids=d.num_res_centroids, in_features=d.in_features,
-                                              out_features=d.out_features, perm=perm, vector_len=16)
+                                              out_features=d.out_features, perm=perm, vector_len=list_vector_len)
         d.lists_stream, d.lists_tab, d.lists_tile_cols = stream.data_ptr(), tab.data_ptr(), int(tcw)
         d._keep = d._keep + (stream, tab)
     if drop_packed:
@@ -481,32 +440,51 @@ def quant_gemv(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, flags: in
     check(rc, "vptq_b200_quant_gemv")
 
 
-class FusedGemv:
-    """Prepared argument arrays for vptq_b200_quant_gemv_multi (layers sharing one input)."""
+class _Launch:
+    """Argument arrays, prepared once, of a launch over 1..MAX_FUSED layers that share one input x."""
+
+    pitch = staticmethod(row_pitch)   # the outputs' row pitch as each entry point has always been given it
 
     def __init__(self, descs, ys):
         n = len(descs)
         if not 1 <= n <= MAX_FUSED or len(ys) != n:
-            raise RuntimeError(f"FusedGemv takes 1..{MAX_FUSED} layers with one output each")
-        if any(d.in_features != descs[0].in_features or d.dtype != descs[0].dtype for d in descs):
-            raise RuntimeError("FusedGemv: the layers must read the same x (same in_features and dtype)")
+            raise RuntimeError(f"{type(self).__name__} takes 1..{MAX_FUSED} layers with one output each")
         self.n, self.descs, self.ys = n, list(descs), list(ys)
-        self.desc_arr = (ctypes.POINTER(LinearDesc) * n)(*[ctypes.pointer(d) for d in descs])
+        self.desc_arr = _desc_array(self.descs)
         self.y_arr = (ctypes.c_void_p * n)(*[y.data_ptr() for y in ys])
-        self.stride_arr = (ctypes.c_int64 * n)(*[y.stride(0) for y in ys])
-        self.separate = False
+        self.stride_arr = (ctypes.c_int64 * n)(*[self.pitch(y) for y in ys])
         self.ws_bytes = None
 
-    def __call__(self, x2d: torch.Tensor, flags: int = 0) -> None:
+    def _ws_bytes(self, tokens: int) -> int:
+        return sum(workspace_bytes(d, tokens, OP_GEMV) for d in self.descs)
+
+    def _launch(self, fn: str, x2d: torch.Tensor, flags: int, *extra) -> int:
+        """lib().fn(n, descs, x, pitch, ys, pitches, tokens, *extra, workspace, its bytes, flags, stream)"""
         dev = x2d.device
+        with _on_device(dev):
+            if self.ws_bytes is None:
+                self.ws_bytes = self._ws_bytes(x2d.shape[0])
+            ws = workspace(dev, self.ws_bytes)
+            return getattr(lib(), fn)(self.n, self.desc_arr, x2d.data_ptr(), row_pitch(x2d), self.y_arr,
+                                      self.stride_arr, x2d.shape[0], *extra, ws.data_ptr(), ws.numel(), flags,
+                                      _stream(dev))
+
+
+class FusedGemv(_Launch):
+    """Prepared argument arrays for vptq_b200_quant_gemv_multi (layers sharing one input)."""
+
+    pitch = staticmethod(lambda y: y.stride(0))
+
+    def __init__(self, descs, ys):
+        super().__init__(descs, ys)
+        if any(d.in_features != descs[0].in_features or d.dtype != descs[0].dtype for d in descs):
+            raise RuntimeError("FusedGemv: the layers must read the same x (same in_features and dtype)")
+        self.separate = False
+
+    def __call__(self, x2d: torch.Tensor, flags: int = 0) -> None:
         if not self.separate:
-            with torch.cuda.device(dev):
-                if self.ws_bytes is None:
-                    self.ws_bytes = sum(workspace_bytes(d, x2d.shape[0], OP_GEMV) for d in self.descs)
-                ws = workspace(dev, self.ws_bytes)   # the list kernel reduces its partial sums through it
-                rc = lib().vptq_b200_quant_gemv_multi_ws(self.n, self.desc_arr, x2d.data_ptr(), row_pitch(x2d),
-                                                         self.y_arr, self.stride_arr, x2d.shape[0], ws.data_ptr(),
-                                                         ws.numel(), flags, _stream(dev))
+            # the list kernel reduces its partial sums through the workspace
+            rc = self._launch("vptq_b200_quant_gemv_multi_ws", x2d, flags)
             if rc != -2:                      # VPTQ_ERR_UNSUPPORTED: these layers cannot share one launch
                 check(rc, "vptq_b200_quant_gemv_multi")
                 return
@@ -519,20 +497,24 @@ def _desc_array(descs):
     return (ctypes.POINTER(LinearDesc) * len(descs))(*[ctypes.pointer(d) for d in descs])
 
 
-def batch_max_tokens(descs) -> int:
-    """vptq_b200_quant_gemv_batch_max_tokens: the largest token count the batched list route takes for these layers
-    (one descriptor or a list of 1..MAX_FUSED reading the same x) on the current device, 0 when they are not eligible.
-    Cached on the first descriptor (the answer depends on the shapes and the device only)."""
+def _max_tokens(fn: str, descs, eligible) -> int:
+    """lib().fn for one descriptor or a list of 1..MAX_FUSED reading the same x, on the current device; 0 unless every
+    descriptor is `eligible`.  Cached on the first descriptor (the answer depends on the shapes and the device only)."""
     descs = [descs] if isinstance(descs, LinearDesc) else list(descs)
-    if not descs or not all(d.lists_stream for d in descs):
+    if not descs or not all(eligible(d) for d in descs):
         return 0
-    idx = torch.cuda.current_device()
-    cache = descs[0].__dict__.setdefault("_batch_max", {})
-    key = (idx,) + tuple(id(d) for d in descs)
+    cache = descs[0].__dict__.setdefault("_max_tokens", {})
+    key = (fn, torch.cuda.current_device()) + tuple(id(d) for d in descs)
     v = cache.get(key)
     if v is None:
-        v = cache[key] = int(lib().vptq_b200_quant_gemv_batch_max_tokens(len(descs), _desc_array(descs)))
+        v = cache[key] = int(getattr(lib(), fn)(len(descs), _desc_array(descs)))
     return v
+
+
+def batch_max_tokens(descs) -> int:
+    """vptq_b200_quant_gemv_batch_max_tokens: the largest token count the batched list route takes for these layers
+    (one descriptor or a list of 1..MAX_FUSED reading the same x) on the current device, 0 when they are not eligible."""
+    return _max_tokens("vptq_b200_quant_gemv_batch_max_tokens", descs, lambda d: d.lists_stream)
 
 
 def quant_gemv_batch(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, flags: int = 0) -> None:
@@ -541,46 +523,23 @@ def quant_gemv_batch(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, fla
     FusedGemvBatch([desc], [y2d])(x2d, flags)
 
 
-class FusedGemvBatch:
+class FusedGemvBatch(_Launch):
     """Prepared argument arrays for vptq_b200_quant_gemv_batch (1..MAX_FUSED layers sharing one input, 1..8 tokens).
     No fall-back: a refusal raises."""
 
-    def __init__(self, descs, ys):
-        n = len(descs)
-        if not 1 <= n <= MAX_FUSED or len(ys) != n:
-            raise RuntimeError(f"FusedGemvBatch takes 1..{MAX_FUSED} layers with one output each")
-        self.n, self.descs, self.ys = n, list(descs), list(ys)
-        self.desc_arr = _desc_array(self.descs)
-        self.y_arr = (ctypes.c_void_p * n)(*[y.data_ptr() for y in ys])
-        self.stride_arr = (ctypes.c_int64 * n)(*[row_pitch(y) for y in ys])
-        self.ws_bytes = None
+    def _ws_bytes(self, tokens: int) -> int:
+        return sum(_ws_bytes_cached(d, 1, OP_GEMV) for d in self.descs)
 
     def __call__(self, x2d: torch.Tensor, flags: int = 0) -> None:
-        dev = x2d.device
-        with _on_device(dev):
-            if self.ws_bytes is None:
-                self.ws_bytes = sum(_ws_bytes_cached(d, 1, OP_GEMV) for d in self.descs)
-            ws = workspace(dev, self.ws_bytes)
-            rc = lib().vptq_b200_quant_gemv_batch(self.n, self.desc_arr, x2d.data_ptr(), row_pitch(x2d), self.y_arr,
-                                                  self.stride_arr, x2d.shape[0], ws.data_ptr(), ws.numel(), flags,
-                                                  _stream(dev))
-        check(rc, "vptq_b200_quant_gemv_batch")
+        check(self._launch("vptq_b200_quant_gemv_batch", x2d, flags), "vptq_b200_quant_gemv_batch")
 
 
 def lists16_max_tokens(descs) -> int:
     """vptq_b200_quant_gemv_lists16_max_tokens: the largest token count (4, 2 or 1) the vector-length-16 list kernel
     takes for these layers (one descriptor or a list of 1..MAX_FUSED reading the same x) on the current device, 0 when
-    they are not eligible.  Cached on the first descriptor (the answer depends on the shapes and the device only)."""
-    descs = [descs] if isinstance(descs, LinearDesc) else list(descs)
-    if not descs or not all(d.lists_stream and d.vector_len == 16 for d in descs):
-        return 0
-    idx = torch.cuda.current_device()
-    cache = descs[0].__dict__.setdefault("_lists16_max", {})
-    key = (idx,) + tuple(id(d) for d in descs)
-    v = cache.get(key)
-    if v is None:
-        v = cache[key] = int(lib().vptq_b200_quant_gemv_lists16_max_tokens(len(descs), _desc_array(descs)))
-    return v
+    they are not eligible."""
+    return _max_tokens("vptq_b200_quant_gemv_lists16_max_tokens", descs,
+                       lambda d: d.lists_stream and d.vector_len == 16)
 
 
 def quant_gemv_lists16(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, flags: int = 0) -> None:
@@ -589,50 +548,29 @@ def quant_gemv_lists16(desc: LinearDesc, x2d: torch.Tensor, y2d: torch.Tensor, f
     FusedGemvLists16([desc], [y2d])(x2d, flags)
 
 
-class FusedGemvLists16:
+class FusedGemvLists16(_Launch):
     """Prepared argument arrays for vptq_b200_quant_gemv_lists16 (1..MAX_FUSED vector-length-16 layers sharing one
     input, 1..4 tokens).  No fall-back: a refusal raises."""
 
-    def __init__(self, descs, ys):
-        n = len(descs)
-        if not 1 <= n <= MAX_FUSED or len(ys) != n:
-            raise RuntimeError(f"FusedGemvLists16 takes 1..{MAX_FUSED} layers with one output each")
-        self.n, self.descs, self.ys = n, list(descs), list(ys)
-        self.desc_arr = _desc_array(self.descs)
-        self.y_arr = (ctypes.c_void_p * n)(*[y.data_ptr() for y in ys])
-        self.stride_arr = (ctypes.c_int64 * n)(*[row_pitch(y) for y in ys])
+    def _ws_bytes(self, tokens: int) -> int:
+        return LISTS16_WORKSPACE_BYTES
 
     def __call__(self, x2d: torch.Tensor, flags: int = 0) -> None:
-        dev = x2d.device
-        with _on_device(dev):
-            ws = workspace(dev, LISTS16_WORKSPACE_BYTES)
-            rc = lib().vptq_b200_quant_gemv_lists16(self.n, self.desc_arr, x2d.data_ptr(), row_pitch(x2d), self.y_arr,
-                                                    self.stride_arr, x2d.shape[0], ws.data_ptr(), ws.numel(), flags,
-                                                    _stream(dev))
-        check(rc, "vptq_b200_quant_gemv_lists16")
+        check(self._launch("vptq_b200_quant_gemv_lists16", x2d, flags), "vptq_b200_quant_gemv_lists16")
 
 
-class FusedGemvTP:
+class FusedGemvTP(_Launch):
     """vptq_b200_quant_gemv_multi_tp: fused layers + the tensor-parallel exchange inside the kernel."""
 
+    pitch = staticmethod(FusedGemv.pitch)
+
     def __init__(self, descs, ys, exchange: TpExchange):
-        n = len(descs)
-        self.n, self.descs, self.ys, self.ex = n, list(descs), list(ys), exchange
-        self.desc_arr = (ctypes.POINTER(LinearDesc) * n)(*[ctypes.pointer(d) for d in descs])
-        self.y_arr = (ctypes.c_void_p * n)(*[y.data_ptr() for y in ys])
-        self.stride_arr = (ctypes.c_int64 * n)(*[y.stride(0) for y in ys])
-        self.ws_bytes = None
+        super().__init__(descs, ys)
+        self.ex = exchange
 
     def __call__(self, x2d: torch.Tensor, flags: int = 0) -> None:
-        dev = x2d.device
-        with torch.cuda.device(dev):
-            if self.ws_bytes is None:
-                self.ws_bytes = sum(workspace_bytes(d, x2d.shape[0], OP_GEMV) for d in self.descs)
-            ws = workspace(dev, self.ws_bytes)
-            rc = lib().vptq_b200_quant_gemv_multi_tp(self.n, self.desc_arr, x2d.data_ptr(), row_pitch(x2d), self.y_arr,
-                                                     self.stride_arr, x2d.shape[0], ctypes.byref(self.ex), ws.data_ptr(),
-                                                     ws.numel(), flags, _stream(dev))
-        check(rc, "vptq_b200_quant_gemv_multi_tp")
+        check(self._launch("vptq_b200_quant_gemv_multi_tp", x2d, flags, ctypes.byref(self.ex)),
+              "vptq_b200_quant_gemv_multi_tp")
 
 
 def tp_untag(tagged: torch.Tensor, y: torch.Tensor, exchange: TpExchange) -> None:

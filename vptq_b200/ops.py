@@ -6,19 +6,16 @@ Function names, argument order and argument meaning are the reference's
 
 * every op runs hand-written sm_90a CUDA through the C ABI (vptq_b200.native); there is no
   torch implementation to fall back to -- CPU tensors raise;
-* routing: fewer than 3 tokens -> fused GEMV (the reference's rule, :213); otherwise the fused
-  dequant->wgmma GEMM instead of `dequant` + `F.linear` (:231-275).  Opt-in (`_batched_decode`,
-  VQuantLinear.set_batched_decode): 2..8 tokens of a layer with index lists -> the batched list kernel.  Opt-in
-  (`_lists_prefill`, VQuantLinear.set_lists_prefill): a decode-only descriptor takes every call the list kernels do
-  not through the GEMM with the weight written from the index lists (include/vptq_b200_lists_dense.h), and its input
-  gradient likewise.  Opt-in (`_list_decode`, VQuantLinear.set_list_decode): 1..lists16_max_tokens tokens of a
-  vector-length-16 layer with index lists -> the v = 16 list kernel (include/vptq_b200_lists16.h); with both
-  opt-ins such a layer may be decode-only too, and its other calls take the GEMM from the lists;
+* routing: `route` alone decides which kernel takes a call -- of one layer, of a fused group of layers
+  (vptq_b200.fuse) or of an input gradient -- from the token count, the alignment of x, the descriptor and the layer's
+  opt-ins (`OptIns`: VQuantLinear.set_batched_decode / set_lists_prefill / set_list_decode).  Without opt-ins it is
+  the reference's rule (fewer than 3 tokens -> fused GEMV, :213), with the fused dequant->wgmma GEMM instead of
+  `dequant` + `F.linear` (:231-275) for larger calls;
 * `argsort(perm)` is not recomputed on every call (the reference does, :208-211).
 """
 from __future__ import annotations
 
-from typing import Optional
+from typing import NamedTuple, Optional
 
 import torch
 from torch.autograd.function import once_differentiable
@@ -26,6 +23,76 @@ from torch.autograd.function import once_differentiable
 from . import native
 
 __all__ = ["dequant", "quant_gemm", "quant_gemv_v2"]
+
+
+class OptIns(NamedTuple):
+    """A VQuantLinear's routing opt-ins: set_batched_decode, set_lists_prefill and set_list_decode."""
+    batched_decode: bool = False
+    lists_prefill: bool = False
+    list_decode: bool = False
+
+
+NO_OPT_INS = OptIns()
+
+# the routes `route` returns
+EMPTY, LISTS16, BATCH, LISTS_GEMM, GEMV, GEMM, DGRAD = (
+    "empty", "lists16", "batch", "lists_gemm", "gemv", "gemm", "dgrad")
+
+
+def route(descs, tokens: int, aligned: bool, opt_ins, vector_len: int = 0, dgrad: bool = False) -> Optional[str]:
+    """The kernel that takes a call of `tokens` rows of x; `aligned`: x starts on a 16-byte boundary.
+
+    One call: `descs` is the layer's descriptor and `opt_ins` its OptIns.  The first rule that holds wins:
+      1. no tokens: EMPTY, no launch;
+      2. list_decode, v = 16, index lists, x aligned or a decode-only descriptor (no packed words; the caller runs it
+         on an aligned copy of x), tokens <= lists16_max_tokens: LISTS16, the v = 16 list kernel;
+      3. batched_decode, 2+ tokens, index lists, x aligned, tokens <= batch_max_tokens: BATCH, the batched list kernel;
+      4. lists_prefill, 2+ tokens, a decode-only descriptor: LISTS_GEMM, the GEMM with the weight from the lists;
+      5. fewer than 3 tokens: GEMV;
+      6. GEMM.
+    A max-token query runs only when every other condition of its rule holds (its answer is cached per descriptor).
+
+    `dgrad`: the route of the input gradient instead: DGRAD (the transposed GEMM) while the descriptor has its packed
+    words, LISTS_GEMM (transposed) for a decode-only one with lists_prefill, None for a decode-only one without.
+
+    A fused group (vptq_b200.fuse): `descs` is a function returning the members' descriptors, called only once a rule
+    needs them (it rebuilds stale ones), `opt_ins` one OptIns per member and `vector_len` the members'.  The rules
+    above apply to the group as one layer: batched_decode and list_decode when every member opted in, "lists_prefill
+    and decode-only" when some member is both, max-token queries for all the descriptors together, and x is never
+    copied.  The group gets GEMV or BATCH (v = 8) or LISTS16 (v = 16) -- the routes that launch the group as one --
+    and None for every other route: each member then runs its own call."""
+    group = not isinstance(opt_ins, OptIns)
+    if group:
+        batched = all(o.batched_decode for o in opt_ins)
+        list_decode = all(o.list_decode for o in opt_ins)
+        lists_prefill = any(o.lists_prefill for o in opt_ins)
+        d = None
+    else:
+        batched, lists_prefill, list_decode = opt_ins
+        d, vector_len = descs, descs.vector_len
+        if dgrad:
+            return DGRAD if d.indices else LISTS_GEMM if lists_prefill else None
+    if tokens == 0:
+        return None if group else EMPTY
+    if list_decode and vector_len == 16:
+        d = d or descs()
+        # a group's query answers 0 when some member has no lists
+        if (group or d.lists_stream) and (aligned or not (group or d.indices)) and \
+                tokens <= native.lists16_max_tokens(d):
+            return LISTS16
+    if group and vector_len == 16:
+        return None           # a v = 16 group launches nothing else as one
+    if batched and tokens >= 2 and aligned:
+        d = d or descs()
+        if (group or d.lists_stream) and tokens <= native.batch_max_tokens(d):
+            return BATCH
+    if group and tokens >= 3:
+        return None           # past the batched kernel a v = 8 group has only the GEMV of 1..2 tokens
+    if lists_prefill and tokens >= 2:
+        d = d or descs()
+        if any(o.lists_prefill and not m.indices for o, m in zip(opt_ins, d)) if group else not d.indices:
+            return None if group else LISTS_GEMM
+    return GEMV if tokens < 3 else GEMM
 
 
 def _desc(*, dtype, indices, centroids, outlier_indices, outlier_centroids, residual_centroids, perm,
@@ -180,25 +247,16 @@ def quant_gemm(
     _desc_cache: Optional[list] = None,
     _drop_packed: bool = False,
     _quant_grad: bool = False,
-    _batched_decode: bool = False,
-    _lists_prefill: bool = False,
-    _list_decode: bool = False,
+    _opt_ins: OptIns = NO_OPT_INS,
 ) -> torch.Tensor:
     """y = x @ W^T + bias for one VPTQ layer (reference: vptq/ops/quant_gemm.py:161-275).
 
     `_quant_grad` (VQuantLinear.set_quant_grad): under grad mode the codebooks, weight_scale and weight_bias that
     require grad get gradients too, also when x does not require grad (vptq_b200_quant_gemm_wgrad).
 
-    `_batched_decode` (VQuantLinear.set_batched_decode): 2..batch_max_tokens tokens of a layer that carries index
-    lists run the batched list kernel (include/vptq_b200_batch.h); every other call is routed as without it.
-
-    `_lists_prefill` (VQuantLinear.set_lists_prefill): on a decode-only descriptor, calls neither list kernel takes
-    and the input gradient run the GEMM with the weight written from the index lists; no effect on a descriptor
-    that still has its packed words.
-
-    `_list_decode` (VQuantLinear.set_list_decode): a kept descriptor of a vector-length-16 layer carries index lists,
-    and 1..lists16_max_tokens tokens run the v = 16 list kernel (include/vptq_b200_lists16.h); every other call is
-    routed as without it.  With `_lists_prefill` too, `_drop_packed` may make that descriptor decode-only."""
+    `_opt_ins` (VQuantLinear.set_batched_decode / set_lists_prefill / set_list_decode): the routes `route` may
+    choose besides the default ones.  With list_decode a kept descriptor of a vector-length-16 layer carries index lists;
+    with lists_prefill as well, `_drop_packed` may make it decode-only."""
     if vector_quant_dim == "in":
         raise ValueError("Not implemented yet.")
     if not is_indice_packed:
@@ -223,7 +281,7 @@ def quant_gemm(
             # a one-off descriptor (reference-style direct call) must not pay for re-bucketing the whole layer:
             # the slice x tile lists are built only when the caller keeps the descriptor (VQuantLinear does)
             lists=None if _desc_cache is not None else False, drop_packed=_drop_packed,
-            lists16=_list_decode and _desc_cache is not None, lists_prefill=_lists_prefill)
+            lists16=_opt_ins.list_decode and _desc_cache is not None, lists_prefill=_opt_ins.lists_prefill)
         if _desc_cache is not None:
             _desc_cache.extend([desc, perm_])   # keep the converted perm alive with the descriptor
     x2d = x.reshape(-1, in_features)
@@ -240,38 +298,31 @@ def quant_gemm(
             if not quant:
                 layer = (indices, centroids, residual_centroids, outlier_indices, outlier_centroids, perm,
                          weight_scale, weight_bias)
-                y = _QuantLinearFn.apply(x2d, bias, keep, out_features, (_batched_decode, _lists_prefill, _list_decode),
-                                         *[t for t in layer if t is not None])
+                y = _QuantLinearFn.apply(x2d, bias, keep, out_features, _opt_ins, *[t for t in layer if t is not None])
             else:
                 others = [t for t in (indices, outlier_indices, perm) if t is not None]
-                y = _QuantLinearWgradFn.apply(x2d, bias, keep, out_features, (_batched_decode, _lists_prefill, _list_decode),
-                                              tuple(n for n, _ in slots), *[t for _, t in slots], *others)
+                y = _QuantLinearWgradFn.apply(x2d, bias, keep, out_features, _opt_ins, tuple(n for n, _ in slots),
+                                              *[t for _, t in slots], *others)
             return y.reshape(*x.shape[:-1], out_features)
-    return _forward(desc, x2d, out_features, _batched_decode, _lists_prefill, _list_decode).reshape(
-        *x.shape[:-1], out_features)
+    return _forward(desc, x2d, out_features, _opt_ins).reshape(*x.shape[:-1], out_features)
 
 
-def _forward(desc, x2d: torch.Tensor, out_features: int, batched: bool = False,
-             lists_prefill: bool = False, list_decode: bool = False) -> torch.Tensor:
+def _forward(desc, x2d: torch.Tensor, out_features: int, opt_ins: OptIns = NO_OPT_INS) -> torch.Tensor:
     tokens = x2d.shape[0]
     y = torch.empty(tokens, out_features, dtype=x2d.dtype, device=x2d.device)
-    if tokens == 0:
-        return y
     aligned = x2d.data_ptr() % 16 == 0
-    if list_decode and desc.vector_len == 16 and desc.lists_stream and (aligned or not desc.indices) and \
-            tokens <= native.lists16_max_tokens(desc):
+    r = route(desc, tokens, aligned, opt_ins)
+    if r is LISTS16:
         # a decode-only descriptor has no other route for these calls: a misaligned x runs on an aligned copy (each
         # token's outputs do not depend on where x lives)
-        xa = x2d if aligned else x2d.clone(memory_format=torch.contiguous_format)
-        native.quant_gemv_lists16(desc, xa, y)
-    elif batched and tokens >= 2 and desc.lists_stream and x2d.data_ptr() % 16 == 0 and \
-            tokens <= native.batch_max_tokens(desc):
+        native.quant_gemv_lists16(desc, x2d if aligned else x2d.clone(memory_format=torch.contiguous_format), y)
+    elif r is BATCH:
         native.quant_gemv_batch(desc, x2d, y)
-    elif lists_prefill and tokens >= 2 and not desc.indices:
+    elif r is LISTS_GEMM:
         native.lists_quant_gemm(desc, x2d, y)
-    elif tokens < 3:
+    elif r is GEMV:
         native.quant_gemv(desc, x2d, y)
-    else:
+    elif r is GEMM:
         native.quant_gemm(desc, x2d, y)
     return y
 
@@ -286,10 +337,10 @@ class _QuantLinearFn(torch.autograd.Function):
     in-place update between forward and backward fails autograd's version check instead of using new weights."""
 
     @staticmethod
-    def forward(ctx, x2d, bias, keep, out_features, route, *layer):
-        ctx.keep, ctx.lists_prefill = keep, route[1]
+    def forward(ctx, x2d, bias, keep, out_features, opt_ins, *layer):
+        ctx.keep, ctx.opt_ins = keep, opt_ins
         ctx.save_for_backward(*layer)
-        return _forward(keep[0], x2d, out_features, *route)
+        return _forward(keep[0], x2d, out_features, opt_ins)
 
     @staticmethod
     @once_differentiable
@@ -301,15 +352,15 @@ class _QuantLinearFn(torch.autograd.Function):
 
 def _input_grads(ctx, desc, dy):
     """(dX, dbias) of y = x W^T + bias for the slots 0 and 1 that need them."""
-    from_lists = not desc.indices and getattr(ctx, "lists_prefill", False)
-    if not desc.indices and not from_lists:
+    r = route(desc, dy.shape[0], True, ctx.opt_ins, dgrad=True)
+    if r is None:
         raise RuntimeError("backward through a decode-only VQuantLinear (prepare(drop_packed=True)): the input "
                            "gradient needs the packed index words, which were freed; reload the checkpoint")
     dx = dbias = None
     if ctx.needs_input_grad[0]:
         dx = torch.empty(dy.shape[0], desc.in_features, dtype=dy.dtype, device=dy.device)
         if dy.shape[0]:
-            if from_lists:        # (set_lists_prefill) Wt written from the index lists
+            if r is LISTS_GEMM:   # Wt written from the index lists
                 native.lists_quant_gemm(desc, dy, dx, native.FLAG_TRANSPOSE)
             else:
                 native.quant_gemm_dgrad(desc, dy, dx)
@@ -328,10 +379,10 @@ class _QuantLinearWgradFn(torch.autograd.Function):
     autograd's version check)."""
 
     @staticmethod
-    def forward(ctx, x2d, bias, keep, out_features, route, names, *layer):
-        ctx.keep, ctx.names, ctx.lists_prefill = keep, names, route[1]
+    def forward(ctx, x2d, bias, keep, out_features, opt_ins, names, *layer):
+        ctx.keep, ctx.names, ctx.opt_ins = keep, names, opt_ins
         ctx.save_for_backward(x2d, *layer)
-        return _forward(keep[0], x2d, out_features, *route)
+        return _forward(keep[0], x2d, out_features, opt_ins)
 
     @staticmethod
     @once_differentiable
