@@ -195,7 +195,7 @@ int gemv_make_plan(const vptq_linear_desc& d, int tokens, const DeviceInfo& dev,
     if (pl.nch > slots) continue;
     pl.cpc = std::max(1, std::min(slots / pl.nch, Ro));
     const int rows_cta = (Ro + pl.cpc - 1) / pl.cpc;
-    const int rows_alloc = rows_cta + rows_cta / 4 + 1;  // cpc may still be clamped below: 25% slack
+    int rows_alloc = rows_cta + rows_cta / 4 + 1;  // cpc may still be clamped below: 25% slack
     // cluster reduce: the leader holds every row's chunk partials
     const size_t part_bytes = size_t(rows_alloc) * pl.nch * pl.nt * v * 4;
     pl.cluster = (pl.nch >= 2 && pl.nch <= 8 && part_bytes <= kMaxClusterPartBytes && tn.cluster != 0) ? 1 : 0;
@@ -241,17 +241,18 @@ int gemv_make_plan(const vptq_linear_desc& d, int tokens, const DeviceInfo& dev,
     std::vector<Shape> shapes;
     for (int st : (a.main_smem ? std::vector<int>{4, 3, 2} : std::vector<int>{2}))
       for (int rep : {a.res_smem ? res_rep_max : 0, a.res_smem ? 1 : 0}) shapes.push_back({st, rep});
-    bool placed = false;
-    for (const Shape& sh : shapes) {
-      if (tn.stages && sh.stages != tn.stages) continue;
-      const size_t need = carve(a.warps, sh.stages, sh.rep);
-      if (need <= size_t(smem_limit)) {
-        pl.threads = a.warps * 32, pl.stages = sh.stages, pl.smem_bytes = uint32_t(need);
-        placed = true;
-        break;
+    auto place = [&]() {
+      for (const Shape& sh : shapes) {
+        if (tn.stages && sh.stages != tn.stages) continue;
+        const size_t need = carve(a.warps, sh.stages, sh.rep);
+        if (need <= size_t(smem_limit)) {
+          pl.threads = a.warps * 32, pl.stages = sh.stages, pl.smem_bytes = uint32_t(need);
+          return true;
+        }
       }
-    }
-    if (!placed) continue;
+      return false;
+    };
+    if (!place()) continue;
 
     // ---- clusters must all be co-resident: a second wave would double the kernel ----------------
     if (pl.cluster && dev.device >= 0) {
@@ -261,7 +262,13 @@ int gemv_make_plan(const vptq_linear_desc& d, int tokens, const DeviceInfo& dev,
                        : -1;
       if (n > 0 && n < pl.cpc) pl.cpc = n;
       const int rows2 = (Ro + pl.cpc - 1) / pl.cpc;
-      if (rows2 > rows_alloc) pl.cluster = 0;
+      if (rows2 > rows_alloc) {
+        // more rows per CTA than the leader's partial-sum table holds: reduce through global memory, and carve the
+        // row-indexed tables (s_wsum, s_wcnt) again for the rows a CTA now owns
+        pl.cluster = 0;
+        rows_alloc = rows2;
+        if (!place()) continue;
+      }
     }
     pl.grid = pl.nch * pl.cpc;
     pl.ws_counters_bytes = kZeroRegionBytes;
