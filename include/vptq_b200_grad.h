@@ -21,9 +21,13 @@
  * Method: terms are added as 64-bit fixed-point integers (red.global.add.u64), so every result is independent of
  * the order the GPU adds them in -- bit-identical from run to run and under CUDA-graph replay.  The unit is a
  * power of two chosen per call on the device from a cheap bound B of the sum of |terms| (unit >= B / 2^61), so
- * no partial sum can overflow.  Each gradient element is rounded once from its sum to the layer's dtype.  If any
- * value of x, dY or G is not finite (including an fp32 element of G that overflows), every requested gradient is
- * NaN (fixed point carries no inf; a loss-scaling loop sees the overflow).  Overflow in the final rounding gives +-inf.
+ * no partial sum can overflow.  Every term is rounded to the unit on its own, and each gradient element is rounded
+ * once, correctly, from its integer sum to the layer's dtype.  If any value of x, dY or G is not finite (including an
+ * fp32 element of G that overflows), or of weight_scale, or -- when d weight_scale is requested -- of any main,
+ * residual or outlier codebook entry, used or not, every requested gradient is NaN (fixed point carries no inf; a
+ * loss-scaling loop sees the overflow).  Without d weight_scale the codebook values are not read, and weight_bias
+ * and bias never are: non-finite values there change no bit.  A sum past the largest finite value gives +-inf with
+ * its sign.
  *
  * Conventions are those of include/vptq_b200.h: the caller allocates outputs and workspace, no call
  * synchronises, every call is CUDA-graph capturable, decode-only descriptors (indices == NULL) are refused, and

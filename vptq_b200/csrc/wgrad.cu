@@ -12,16 +12,17 @@
 //                 bound below is the same on every run); max |C|, |R|, |Col| (order-free atomicMax).
 //   2. units      one CTA: the bounds B_cb = sum |s_f G| (>=), B_bias = sum |G|, B_scale = B_bias max|Wq| in fp64
 //                 and from them the power-of-two units 2^e >= B / 2^61 of the three fixed-point sums; a non-finite
-//                 bound marks the call non-finite.
+//                 bound (B_scale included: inf / NaN in a codebook while d weight_scale is wanted) marks the call
+//                 non-finite.
 //   3. scatter    a thread owns one column and 16 index rows: it decodes the field of every (r, c) like the dequant
 //                 kernels do, adds s_f G[o][f] as a 64-bit fixed-point integer into dC[k][e] (red.global.add.u64)
 //                 and dR[kr][e] (a per-CTA shared-memory table for small residual codebooks, flushed once), and
-//                 forms its column's fp32 partial sums of G Wq and G, added once in fixed point to
-//                 d weight_scale[f] / d weight_bias[f].
-//   4. finish     integer * 2^e in fp64, rounded once to the layer's dtype (NaN everywhere for a non-finite call).
+//                 rounds each term G Wq and G of its column to its unit as well, summing them in registers and
+//                 adding the sums once to d weight_scale[f] / d weight_bias[f].
+//   4. finish     integer * 2^e rounded once to the layer's dtype: the int64 goes to fp64 with round-to-odd, so
+//                 the fp64 -> 16-bit conversion is the only rounding (NaN everywhere for a non-finite call).
 // Integer addition is associative, so the results do not depend on the order in which the GPU adds the terms:
-// bit-identical from run to run and under CUDA-graph replay.  Each scatter thread's fp32 partial sums cover a
-// fixed set of elements, so they are reproducible too.
+// bit-identical from run to run and under CUDA-graph replay.
 #include <algorithm>
 #include <cmath>
 
@@ -133,7 +134,11 @@ __global__ void __launch_bounds__(256) wg_row_stats(const T* __restrict__ p, int
   }
 }
 
-// *out = max(*out, max |p[g][i]|) over groups g < groups, i < n (bit pattern of a non-negative float)
+// max that keeps NaN (fmaxf drops it): |NaN| wins over every number
+__device__ __forceinline__ float max_nan(float a, float b) { return (b > a || b != b) ? b : a; }
+
+// *out = max(*out, max |p[g][i]|) over groups g < groups, i < n (bit pattern of a non-negative float; a positive NaN
+// orders above +inf, so a NaN entry reaches wg_units)
 template <typename T>
 __global__ void __launch_bounds__(256) wg_absmax(const T* __restrict__ p, int groups, int64_t n, int64_t stride,
                                                  uint32_t* out) {
@@ -141,11 +146,11 @@ __global__ void __launch_bounds__(256) wg_absmax(const T* __restrict__ p, int gr
   const int64_t total = int64_t(groups) * n;
   for (int64_t i = int64_t(blockIdx.x) * 256 + threadIdx.x; i < total; i += int64_t(gridDim.x) * 256) {
     const int64_t g = i / n;
-    m = fmaxf(m, fabsf(DT<T>::to_float(p[g * stride + (i - g * n)])));
+    m = max_nan(m, fabsf(DT<T>::to_float(p[g * stride + (i - g * n)])));
   }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-  if ((threadIdx.x & 31) == 0 && m > 0.f) atomicMax(out, __float_as_uint(m));
+  for (int o = 16; o > 0; o >>= 1) m = max_nan(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0 && __float_as_uint(m) != 0u) atomicMax(out, __float_as_uint(m));
 }
 
 __device__ int unit_exponent(double bound) {
@@ -173,9 +178,12 @@ __global__ void __launch_bounds__(256) wg_units(const double* __restrict__ a, co
   }
   if (threadIdx.x == 0) {
     const double bc = r1[0], bb = r2[0];
-    const double mwq = fmax(double(__uint_as_float(hdr->max_c)) + double(__uint_as_float(hdr->max_r)),
-                            double(__uint_as_float(hdr->max_col)));
-    hdr->nonfinite = !(isfinite(bc) && isfinite(bb));
+    const double mc = double(__uint_as_float(hdr->max_c)) + double(__uint_as_float(hdr->max_r));
+    const double mo = double(__uint_as_float(hdr->max_col));
+    const double mwq = fmax(mc, mo);
+    // the maxima are 0 unless d weight_scale is wanted: a non-finite codebook matters only then.  Both are tested,
+    // since fmax drops a NaN.
+    hdr->nonfinite = !(isfinite(bc) && isfinite(bb) && isfinite(bb * mc) && isfinite(bb * mo));
     hdr->e_cb = unit_exponent(bc);
     hdr->e_bias = unit_exponent(bb);
     hdr->e_scale = unit_exponent(bb * mwq);
@@ -345,6 +353,18 @@ __device__ __forceinline__ __half from_double<__half>(double v) { return __doubl
 template <>
 __device__ __forceinline__ __nv_bfloat16 from_double<__nv_bfloat16>(double v) { return __double2bfloat16(v); }
 
+// int64 -> fp64 rounded to odd: exact up to 2^53; above, truncated with the dropped bits ORed into the last bit.  With
+// 53 >= p + 2 significant bits, rounding that value to the p-bit 16-bit type (p <= 11) rounds the integer itself
+// correctly: a single rounding.  (A plain conversion rounds to nearest first and can land on a tie of the 16-bit type.)
+__device__ __forceinline__ double ll_to_double_odd(long long v) {
+  const unsigned long long m = v < 0 ? 0ull - static_cast<unsigned long long>(v) : static_cast<unsigned long long>(v);
+  if (m <= (1ull << 53)) return double(v);
+  const int drop = 11 - __clzll(static_cast<long long>(m));   // bits below the 53 kept (m < 2^63)
+  const unsigned long long keep = (m >> drop) | ((m & ((1ull << drop) - 1ull)) != 0ull);
+  const double r = ldexp(double(keep), drop);                // exact: keep < 2^53
+  return v < 0 ? -r : r;
+}
+
 // out[row * out_stride + col] = acc[row * row_len + col] * 2^e, rounded once (NaN for a non-finite call)
 template <typename T>
 __global__ void __launch_bounds__(256) wg_finish(const unsigned long long* __restrict__ acc, int64_t n,
@@ -355,7 +375,7 @@ __global__ void __launch_bounds__(256) wg_finish(const unsigned long long* __res
   for (int64_t i = int64_t(blockIdx.x) * 256 + threadIdx.x; i < n; i += int64_t(gridDim.x) * 256) {
     const int64_t row = i / row_len, col = i - row * row_len;
     const double v = h.nonfinite ? __longlong_as_double(0x7ff8000000000000ll)
-                                 : ldexp(double(static_cast<long long>(acc[i])), e);
+                                 : ldexp(ll_to_double_odd(static_cast<long long>(acc[i])), e);
     out[row * out_stride + col] = from_double<T>(v);
   }
 }
